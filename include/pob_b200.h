@@ -67,6 +67,7 @@ typedef struct {
     uint32_t expand_group;     /* instances materialised per expand launch (<= n_slots) */
     uint32_t opt_level;        /* 0 = circom --O0 witness (every signal), 1 = reduced witness (POB_CREATE_O1) */
     uint64_t n_signals_o0;     /* witness entries of the --O0 layout (== n_signals when opt_level == 0) */
+    uint32_t n_compressed_slots; /* of the n_slots, those the driver made compressible memory (Compute Data Compression) */
 } pob_desc;
 
 /* `hcreate` argument of pob_create / pob_layout_info / pob_constraint_info: bit 0 = creation-order sub-component numbering

@@ -8,6 +8,7 @@
 // k_eval on the highest-priority stream (its 32-CTA grid must get SMs while the expand grid of hundreds of thousands of
 // CTAs drains), expand on the lowest.  Slots are freed by the consumer (pob_release; stream-ordered, so the stall happens
 // on the GPU), by the built-in digest consumer, or -- only when the caller says POB_RUN_DISCARD -- at once.
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <fcntl.h>
 #include <unistd.h>
@@ -42,6 +43,46 @@ static const char *tune_env(const char *name) {
     (void)name; return nullptr;
 #endif
 }
+
+// Witness slots come from the driver's virtual-memory API so that they can be compressible memory (Compute Data
+// Compression): 95.8 % of a main-shape witness is 32-byte entries holding a single 0/1 byte, which L2 compresses before it
+// writes the line to DRAM.  The entry points are looked up through the runtime, so the library does not link libcuda.
+#define CUD(call) do { CUresult r_ = (call); if (r_ != CUDA_SUCCESS) throw std::runtime_error(std::string(#call) + ": CUresult " + std::to_string((int)r_)); } while (0)
+namespace {
+struct DriverVmm {
+    decltype(&::cuDeviceGet) deviceGet = nullptr;
+    decltype(&::cuDeviceGetAttribute) deviceGetAttribute = nullptr;
+    decltype(&::cuMemGetAllocationGranularity) granularity = nullptr;
+    decltype(&::cuMemCreate) create = nullptr;
+    decltype(&::cuMemGetAllocationPropertiesFromHandle) properties = nullptr;
+    decltype(&::cuMemAddressReserve) reserve = nullptr;
+    decltype(&::cuMemMap) map = nullptr;
+    decltype(&::cuMemSetAccess) setAccess = nullptr;
+    decltype(&::cuMemUnmap) unmap = nullptr;
+    decltype(&::cuMemRelease) release = nullptr;
+    decltype(&::cuMemAddressFree) addressFree = nullptr;
+};
+template <class F> static void driver_entry(const char *name, F &fn) {
+    void *p = nullptr; cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
+    CU(cudaGetDriverEntryPointByVersion(name, &p, 12000, cudaEnableDefault, &q));
+    if (q != cudaDriverEntryPointSuccess || !p) throw std::runtime_error(std::string("driver entry point ") + name + " not found");
+    fn = reinterpret_cast<F>(p);
+}
+static const DriverVmm &vmm() {
+    static const DriverVmm d = [] {
+        DriverVmm v;
+        driver_entry("cuDeviceGet", v.deviceGet); driver_entry("cuDeviceGetAttribute", v.deviceGetAttribute);
+        driver_entry("cuMemGetAllocationGranularity", v.granularity); driver_entry("cuMemCreate", v.create);
+        driver_entry("cuMemGetAllocationPropertiesFromHandle", v.properties); driver_entry("cuMemAddressReserve", v.reserve);
+        driver_entry("cuMemMap", v.map); driver_entry("cuMemSetAccess", v.setAccess); driver_entry("cuMemUnmap", v.unmap);
+        driver_entry("cuMemRelease", v.release); driver_entry("cuMemAddressFree", v.addressFree);
+        return v;
+    }();
+    return d;
+}
+// one witness slot: physical allocation, its own virtual address range, the mapping; pob_destroy undoes what is set
+struct VmSlot { CUmemGenericAllocationHandle mem = 0; CUdeviceptr va = 0; bool mapped = false; };
+}  // namespace
 
 // =============================================================================================================
 // exporter: resident witness -> host (.wtns image), several copy streams into a pinned staging ring, file I/O on a
@@ -139,6 +180,7 @@ struct pob_handle {
     uint32_t chunk = 0; uint64_t store_stride = 0; uint64_t *d_stores = nullptr; uint64_t *d_inputs = nullptr;
     // witness slots
     std::vector<uint64_t *> slots;
+    std::vector<VmSlot> slot_vm; size_t slot_bytes = 0; uint32_t n_compressed_slots = 0;   // slots[s] is mapped at slot_vm[s].va
     std::vector<int64_t> slot_owner;              // instance (of the current / last batch) whose witness the slot holds, -1 = none
     std::vector<cudaEvent_t> slot_rel_ev; std::vector<uint8_t> slot_rel_pending;   // stream-ordered release by the consumer
     std::vector<uint32_t> last_status; uint32_t last_n = 0;
@@ -514,7 +556,15 @@ void pob_destroy(pob_handle *h) {
                     (void *)h->d_tiles, (void *)h->d_invtab, (void *)h->d_round_desc, (void *)h->d_stores, (void *)h->d_inputs, (void *)h->d_status,
                     (void *)h->d_outputs, (void *)h->d_digests, (void *)h->d_witptr, (void *)h->d_planinst, (void *)h->d_staged, (void *)h->d_prof, (void *)h->d_block_base})
         if (p) cudaFree(p);
-    for (uint64_t *s : h->slots) cudaFree(s);
+    if (!h->slot_vm.empty()) {
+        const DriverVmm &D = vmm();
+        cudaDeviceSynchronize();                  // a consumer's stream may still read a slot (cudaFree used to wait for it)
+        for (const VmSlot &s : h->slot_vm) {
+            if (s.mapped) D.unmap(s.va, h->slot_bytes);
+            if (s.va) D.addressFree(s.va, h->slot_bytes);
+            if (s.mem) D.release(s.mem);
+        }
+    }
     for (void *p : {(void *)h->h_status, (void *)h->h_outputs, (void *)h->h_digests, (void *)h->h_witptr, (void *)h->h_planinst}) if (p) cudaFreeHost(p);
     for (cudaEvent_t e : h->ev_pool) cudaEventDestroy(e);
     for (cudaEvent_t e : h->slot_rel_ev) cudaEventDestroy(e);
@@ -582,12 +632,42 @@ int pob_create(const char *main_name, const uint64_t *params, int nparams, int h
         if (P.opt_level) chunk = std::max<uint32_t>(chunk, 128);
         chunk -= chunk % 32;
         if (const char *v = tune_env("POB_EVAL_CHUNK")) chunk = (uint32_t)std::max(1, atoi(v));
+        // each slot is compressible memory where the device supports it; what the driver grants is counted per slot
+        const DriverVmm &D = vmm();
+        CUdevice cdev = 0; CUD(D.deviceGet(&cdev, device));
+        int compress = 0; CUD(D.deviceGetAttribute(&compress, CU_DEVICE_ATTRIBUTE_GENERIC_COMPRESSION_SUPPORTED, cdev));
+        if (const char *v = tune_env("POB_SLOT_COMPRESS")) compress = compress && atoi(v) != 0;
+        CUmemAllocationProp mprop{};
+        mprop.type = CU_MEM_ALLOCATION_TYPE_PINNED; mprop.location.type = CU_MEM_LOCATION_TYPE_DEVICE; mprop.location.id = device;
+        mprop.allocFlags.compressionType = compress ? CU_MEM_ALLOCATION_COMP_GENERIC : CU_MEM_ALLOCATION_COMP_NONE;
+        size_t gran = 0; CUD(D.granularity(&gran, &mprop, CU_MEM_ALLOC_GRANULARITY_RECOMMENDED));
+        const size_t vbytes = (wbytes + gran - 1) / gran * gran;
         const uint64_t ring_bytes_per_inst = pob_handle::RING * (h->store_stride * 8 + (uint64_t)P.n_inputs * 32);
         uint64_t budget = (uint64_t)(free_b * 0.8);
-        uint64_t nslots = budget > chunk * ring_bytes_per_inst ? (budget - chunk * ring_bytes_per_inst) / wbytes : 0;
+        uint64_t nslots = budget > chunk * ring_bytes_per_inst ? (budget - chunk * ring_bytes_per_inst) / vbytes : 0;
         if (max_slots && nslots > max_slots) nslots = max_slots;
         if (nslots > 4096) nslots = 4096;
         if (nslots == 0) throw std::runtime_error("not even one witness slot fits in free HBM");
+        h->chunk = chunk;
+        CU(cudaMalloc(&h->d_stores, (size_t)pob_handle::RING * chunk * h->store_stride * 8));
+        CU(cudaMalloc(&h->d_inputs, std::max<size_t>(32, (size_t)pob_handle::RING * chunk * P.n_inputs * 32)));
+        h->slot_bytes = vbytes;
+        CUmemAccessDesc acc{}; acc.location = mprop.location; acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+        for (uint64_t s = 0; s < nslots; s++) {
+            CUmemGenericAllocationHandle mem = 0;
+            const CUresult r = D.create(&mem, vbytes, &mprop, 0);
+            if (r == CUDA_ERROR_OUT_OF_MEMORY && s > 0) break;      // the compression backing store may cost HBM: keep the slots made
+            if (r == CUDA_ERROR_OUT_OF_MEMORY) throw std::runtime_error("not even one witness slot fits in free HBM (cuMemCreate)");
+            if (r != CUDA_SUCCESS) throw std::runtime_error("cuMemCreate: CUresult " + std::to_string((int)r));
+            h->slot_vm.push_back(VmSlot{}); VmSlot &m = h->slot_vm.back(); m.mem = mem;
+            CUD(D.reserve(&m.va, vbytes, gran, 0, 0));
+            CUD(D.map(m.va, vbytes, 0, m.mem, 0)); m.mapped = true;
+            CUD(D.setAccess(m.va, vbytes, &acc, 1));
+            CUmemAllocationProp got{}; CUD(D.properties(&got, m.mem));
+            if (got.allocFlags.compressionType == CU_MEM_ALLOCATION_COMP_GENERIC) h->n_compressed_slots++;
+            h->slots.push_back(reinterpret_cast<uint64_t *>(m.va));
+        }
+        nslots = h->slots.size();
         // expand group: ~100 GB of witness per launch pair (main_proof_of_burn: 16 witnesses; Spend: up to the whole chunk)
         h->xgroup = (uint32_t)std::min<uint64_t>(std::min<uint64_t>(nslots, chunk), std::max<uint64_t>(16, (100ull << 30) / wbytes));
         if (const char *v = tune_env("POB_EVAL_THREADS")) h->eval_threads = atoi(v);
@@ -615,10 +695,6 @@ int pob_create(const char *main_name, const uint64_t *params, int nparams, int h
             CU(cudaFuncSetAttribute(k_expand_round<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->round_dyn_smem));
         }
         if (const char *v = tune_env("POB_EXPAND_GROUP")) h->xgroup = (uint32_t)std::max(1, std::min<int>(atoi(v), (int)std::min<uint64_t>(nslots, chunk)));
-        h->chunk = chunk;
-        CU(cudaMalloc(&h->d_stores, (size_t)pob_handle::RING * chunk * h->store_stride * 8));
-        CU(cudaMalloc(&h->d_inputs, std::max<size_t>(32, (size_t)pob_handle::RING * chunk * P.n_inputs * 32)));
-        for (uint64_t s = 0; s < nslots; s++) { uint64_t *p = nullptr; CU(cudaMalloc(&p, wbytes)); h->slots.push_back(p); }
         if (h->eval_l2_mb) {       // tuning: keep (part of) the store ring persisting in L2 for the kernels of the eval stream
             const size_t ring = (size_t)pob_handle::RING * chunk * h->store_stride * 8, carve = (size_t)h->eval_l2_mb << 20;
             CU(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, carve));
@@ -648,7 +724,8 @@ int pob_witness_map(const pob_handle *h, uint32_t *map) {
 
 int pob_describe(const pob_handle *h, pob_desc *out) {
     if (!h || !out) return fail(POB_E_BAD_ARG, "pob_describe: null argument");
-    fill_desc(h->P, out); out->n_slots = (uint32_t)h->slots.size(); out->chunk = h->chunk; out->expand_group = h->xgroup; return POB_OK;
+    fill_desc(h->P, out); out->n_slots = (uint32_t)h->slots.size(); out->chunk = h->chunk; out->expand_group = h->xgroup;
+    out->n_compressed_slots = h->n_compressed_slots; return POB_OK;
 }
 
 void *pob_alloc_pinned(uint64_t bytes) { void *p = nullptr; if (cudaMallocHost(&p, bytes ? bytes : 1) != cudaSuccess) { g_err = "cudaMallocHost failed"; return nullptr; } return p; }

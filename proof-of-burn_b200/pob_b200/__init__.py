@@ -43,7 +43,7 @@ class Desc(ctypes.Structure):
                 ("witness_bytes", ctypes.c_uint64), ("wtns_file_bytes", ctypes.c_uint64), ("store_bytes", ctypes.c_uint64),
                 ("n_ops", ctypes.c_uint64), ("n_absorbs", ctypes.c_uint32), ("n_levels", ctypes.c_uint32),
                 ("n_tiles", ctypes.c_uint32), ("n_slots", ctypes.c_uint32), ("chunk", ctypes.c_uint32), ("expand_group", ctypes.c_uint32),
-                ("opt_level", ctypes.c_uint32), ("n_signals_o0", ctypes.c_uint64)]
+                ("opt_level", ctypes.c_uint32), ("n_signals_o0", ctypes.c_uint64), ("n_compressed_slots", ctypes.c_uint32)]
 
     def as_dict(self):
         return {k: int(getattr(self, k)) for k, _ in self._fields_}
