@@ -12,10 +12,11 @@
 //             inputs; the ones that need a field inversion are batch-inverted (one inversion per worker thread) by a state machine
 //             that advances INV_STEPS iterations per level.
 //   k_expand_round / k_expand_codes  the HBM-bound kernels: materialise every witness entry as a 32-byte little-endian
-//             field element with two 128-bit stores (STG.E.128).  Algorithmic bytes = 32 * n_signals per instance
-//             (6.909 GB for main_proof_of_burn).  KeccakfRound blocks (95.8 %) are driven by 8-byte group descriptors
-//             and the round's lane words, everything else by one 32-bit code per entry; both kernels stage their
-//             tables in shared memory with TMA bulk copies (cp.async.bulk + mbarrier).
+//             field element, one 16-byte half per thread and 128-bit store (STG.E.128), so that a warp's store covers 512
+//             contiguous bytes.  Algorithmic bytes = 32 * n_signals per instance (6.909 GB for main_proof_of_burn).
+//             KeccakfRound blocks (95.8 %) are driven by 8-byte group descriptors and the round's lane words, everything
+//             else by one 32-bit code per entry; both kernels stage their tables in shared memory with TMA bulk copies
+//             (cp.async.bulk + mbarrier).
 //   k_check_eq / k_check_kc / k_check_r1  every constraint of the circuit evaluated against a resident witness (cons_check.h).
 //   k_check_rounds  layout-independent check of every KeccakfRound block (textbook round on its in/out signals).
 //   k_digest  64-bit digest of a materialised witness (parity tests at full size; the built-in on-GPU consumer).
@@ -344,18 +345,10 @@ __global__ void __maxnreg__(THREADS == 1024 ? 64 : 104) k_eval(const EvalArgs a)
     }
 }
 
-// One 32-byte entry as two 128-bit stores (STG.E.128; sm_90 has no 256-bit store).  No "memory" clobber on purpose: the
+// Half a 32-byte entry as one 128-bit store (STG.E.128; sm_90 has no 256-bit store).  No "memory" clobber on purpose: the
 // compiler must be free to hoist the next entries' loads above it so that several loads are in flight per thread (the
-// witness is written, never read, here).
-__device__ __forceinline__ void st256(uint64_t *p, uint64_t a, uint64_t b, uint64_t c, uint64_t d) {
-    asm volatile("st.global.v2.b64 [%0], {%1, %2};\n\tst.global.v2.b64 [%0+16], {%3, %4};" ::"l"(p), "l"(a), "l"(b), "l"(c), "l"(d));
-}
-
-// streaming flavour: evict-first in L2, so that the witness write stream does not flush the eval kernel's working set out of L2
-__device__ __forceinline__ void st256cs(uint64_t *p, uint64_t a, uint64_t b, uint64_t c, uint64_t d) {
-    asm volatile("st.global.cs.v2.b64 [%0], {%1, %2};\n\tst.global.cs.v2.b64 [%0+16], {%3, %4};" ::"l"(p), "l"(a), "l"(b), "l"(c), "l"(d));
-}
-// half an entry (k_expand_round)
+// witness is written, never read, here).  The streaming flavour is evict-first in L2, so that the witness write stream does
+// not flush the eval kernel's working set out of L2.
 __device__ __forceinline__ void st128(uint64_t *p, uint64_t a, uint64_t b) { asm volatile("st.global.v2.b64 [%0], {%1, %2};" ::"l"(p), "l"(a), "l"(b)); }
 __device__ __forceinline__ void st128cs(uint64_t *p, uint64_t a, uint64_t b) { asm volatile("st.global.cs.v2.b64 [%0], {%1, %2};" ::"l"(p), "l"(a), "l"(b)); }
 
@@ -418,10 +411,11 @@ __global__ void __launch_bounds__(T) k_expand_round(const ExpandArgs a) {
 // k_expand_codes: grid = (instances in the group, code tiles) -- INSTANCE-major, so that a tile's code stream is fetched
 // from DRAM once and served from L2 to the other witnesses of the group.  One 32-bit code per entry.  The tile's code stream
 // (<= 32 KiB, contiguous) is brought into shared memory by ONE TMA bulk copy, so the first of the two dependent memory hops of
-// an entry (code -> store word / value -> witness) costs a shared-memory read; the gathers of UG entries per thread are then in
-// flight together, ahead of the stores.
-template <int UG>
-__global__ void __launch_bounds__(256, UG == 4 ? 5 : 4) k_expand_codes(const ExpandArgs a) {
+// an entry (code -> store word / value -> witness) costs a shared-memory read; the gathers of UG half entries per thread are
+// then in flight together, ahead of the stores.  Launched with unused dynamic shared memory so that three CTAs are resident
+// per SM (pob_b200.cu codes_dyn_smem).
+__global__ void __launch_bounds__(256, 3) k_expand_codes(const ExpandArgs a) {
+    constexpr int UG = 4;
     const uint32_t gi = a.inst[blockIdx.x];
     if (a.status[gi] != 0) return;
     const Tile t = a.tiles[a.tile0 + blockIdx.y];
@@ -436,23 +430,27 @@ __global__ void __launch_bounds__(256, UG == 4 ? 5 : 4) k_expand_codes(const Exp
     if (threadIdx.x == 0) { mbar_expect_tx(&s_bar, bytes); tma_load_1d(sC, a.codes + (t.code_off - off4), bytes, &s_bar); }
     mbar_wait(&s_bar, 0);
     const Code *c = sC + off4;
-    for (uint32_t base = threadIdx.x; base < t.n; base += 256 * UG) {
-        uint64_t v[UG][4];
+    // one 16-byte half u of the tile per thread and store, as in k_expand_round: entry u / 2, half h = u & 1 (the same for every
+    // u of a thread).  Lanes 2j and 2j+1 read the same code word (a shared-memory broadcast); a warp's stores cover 512
+    // contiguous bytes, and a value slot or constant (32-byte aligned) is gathered by a lane pair as one whole sector, one
+    // 128-bit load per lane.  A 0/1 bit or a small constant has a zero upper half: that lane stores zeros and gathers nothing.
+    const uint32_t n2 = 2 * t.n, h = threadIdx.x & 1u;
+    for (uint32_t base = threadIdx.x; base < n2; base += 256 * UG) {
+        uint64_t v[UG][2];
 #pragma unroll
-        for (int u = 0; u < UG; u++) {
-            const uint32_t k = base + 256 * u;
-            const Code cd = k < t.n ? c[k] : 0u;
+        for (int j = 0; j < UG; j++) {
+            const uint32_t u = base + 256 * j;
+            const Code cd = u < n2 ? c[u >> 1] : 0u;
             const uint32_t kind = code_kind(cd), p = code_payload(cd);
-            v[u][1] = v[u][2] = v[u][3] = 0;
-            if (kind == K_BIT) v[u][0] = (Ub[p >> 6] >> (p & 63)) & 1ull;
-            else if (kind == K_CONST) v[u][0] = p;
-            else {
+            v[j][0] = v[j][1] = 0;
+            if (kind == K_VAL || kind == K_KONST) {
                 const uint64_t *s = (kind == K_VAL) ? U + a.val_base + 4ull * p : reinterpret_cast<const uint64_t *>(a.konst + p);
-                v[u][0] = s[0]; v[u][1] = s[1]; v[u][2] = s[2]; v[u][3] = s[3];
-            }
+                const ulonglong2 q = reinterpret_cast<const ulonglong2 *>(s)[h];
+                v[j][0] = q.x; v[j][1] = q.y;
+            } else if (!h) v[j][0] = (kind == K_BIT) ? (Ub[p >> 6] >> (p & 63)) & 1ull : p;
         }
 #pragma unroll
-        for (int u = 0; u < UG; u++) { const uint32_t k = base + 256 * u; if (k < t.n) { if (a.cs) st256cs(W + 4ull * k, v[u][0], v[u][1], v[u][2], v[u][3]); else st256(W + 4ull * k, v[u][0], v[u][1], v[u][2], v[u][3]); } }
+        for (int j = 0; j < UG; j++) { const uint32_t u = base + 256 * j; if (u < n2) { if (a.cs) st128cs(W + 2ull * u, v[j][0], v[j][1]); else st128(W + 2ull * u, v[j][0], v[j][1]); } }
     }
 }
 

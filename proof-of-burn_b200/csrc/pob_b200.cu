@@ -196,7 +196,10 @@ struct pob_handle {
     // k_expand_round is launched with 85 KiB of (unused) dynamic shared memory so that only TWO of its CTAs are resident
     // per SM (the SM has 228 KB): fewer concurrent write streams give the DRAM controllers longer same-row bursts
     uint32_t round_dyn_smem = 85 * 1024;
-    uint32_t round_threads = 256, codes_dyn_smem = 0, codes_ug = 4, codes_overlap = 0; bool serialize = false;   // changed by POB_TUNING knobs only
+    // k_expand_codes likewise carries 24 KiB next to its 32 KiB code buffer: THREE resident CTAs per SM instead of six.  With
+    // half-entry stores the code tiles take 68 instead of 85 ms per 512 witnesses that way (H100, DESIGN.md §2.3)
+    uint32_t codes_dyn_smem = 24 * 1024;
+    uint32_t round_threads = 256, codes_overlap = 0; bool serialize = false;   // changed by POB_TUNING knobs only
     int eval_threads = 512; uint32_t eval_cluster = 0, eval_prefetch = 0;   // k_eval: threads per CTA; CTAs per instance (0 = chosen per launch)
     uint32_t pos_konst_bytes = 0, levels_bytes = 0, eval_smem = 0;
     bool skip_eval = false;                     // tuning: evaluate only the first two chunks, then re-expand their stores (isolates the cost of concurrency)
@@ -363,15 +366,14 @@ static void enqueue_group(pob_handle *h, uint32_t g) {
     // launch 1: KeccakfRound tiles, tile-major (each CTA's tables are staged in shared memory);
     // launch 2: code tiles, INSTANCE-major, so that a tile's code stream is fetched from DRAM once and
     // served from L2 to the other witnesses of the group
-    // codes_overlap: the code-tile kernel (latency-bound gathers) runs on a second stream NEXT TO the round kernel (bandwidth-bound)
+    // codes_overlap: the code-tile kernel (gathers from the instance store) runs on a second stream NEXT TO the round kernel (bandwidth-bound)
     // instead of after it; 1 = round kernel launched first, 2 = code kernel launched first
     const uint32_t n_round = h->n_round_tiles, n_code = (uint32_t)P.tiles.size() - n_round;
     const bool fork = h->codes_overlap && n_round && n_code;
     cudaStream_t s_codes = fork ? h->s_exp2 : h->s_exp;
     auto launch_codes = [&]() {
         xa.tile0 = n_round;
-        if (h->codes_ug == 8) k_expand_codes<8><<<dim3(gc, n_code), 256, h->codes_dyn_smem, s_codes>>>(xa);
-        else k_expand_codes<4><<<dim3(gc, n_code), 256, h->codes_dyn_smem, s_codes>>>(xa);
+        k_expand_codes<<<dim3(gc, n_code), 256, h->codes_dyn_smem, s_codes>>>(xa);
         B.T.other_launches++;
     };
     if (fork) { CU(cudaEventRecord(h->ev_fork, h->s_exp)); CU(cudaStreamWaitEvent(h->s_exp2, h->ev_fork, 0)); if (h->codes_overlap == 2) launch_codes(); }
@@ -685,9 +687,10 @@ int pob_create(const char *main_name, const uint64_t *params, int nparams, int h
         if (const char *v = tune_env("POB_SERIALIZE")) h->serialize = atoi(v) != 0;
         if (const char *v = tune_env("POB_EXPAND_SMEM_KB")) h->round_dyn_smem = (uint32_t)atoi(v) * 1024u;
         if (const char *v = tune_env("POB_EXPAND_THREADS")) h->round_threads = (uint32_t)atoi(v);
-        if (const char *v = tune_env("POB_CODES_UG")) h->codes_ug = (uint32_t)atoi(v);
         if (const char *v = tune_env("POB_CODES_OVERLAP")) h->codes_overlap = (uint32_t)atoi(v);
-        if (const char *v = tune_env("POB_CODES_SMEM_KB")) { h->codes_dyn_smem = (uint32_t)atoi(v) * 1024u; if (h->codes_dyn_smem > 48 * 1024) { CU(cudaFuncSetAttribute(k_expand_codes<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->codes_dyn_smem)); CU(cudaFuncSetAttribute(k_expand_codes<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->codes_dyn_smem)); } }
+        if (const char *v = tune_env("POB_CODES_SMEM_KB")) h->codes_dyn_smem = (uint32_t)atoi(v) * 1024u;
+        // static (the 32 KiB code buffer) + dynamic shared memory above 48 KiB needs the opt-in
+        CU(cudaFuncSetAttribute(k_expand_codes, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->codes_dyn_smem));
         if (h->round_dyn_smem > 48 * 1024) {
             CU(cudaFuncSetAttribute(k_expand_round<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->round_dyn_smem));
             CU(cudaFuncSetAttribute(k_expand_round<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->round_dyn_smem));

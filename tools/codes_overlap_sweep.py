@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Does the code-tile kernel (4.1 % of the bytes, latency-bound gathers) hide next to the round kernel (bandwidth-
+"""Does the code-tile kernel (4.1 % of the bytes, gathers from the instance stores) hide next to the round kernel (bandwidth-
 bound) when both run at the same time on two streams?  (TUNING build: POB_CODES_OVERLAP = 0 after it, 1 next to it / round kernel
 launched first, 2 next to it / code kernel launched first; POB_EXPAND_SMEM_KB = the round kernel's shared-memory cap, which decides
 how many code CTAs fit beside its two resident CTAs.)  Staged 512-instance batch of the main shape, digests compared."""
