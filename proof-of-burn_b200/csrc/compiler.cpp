@@ -2263,7 +2263,7 @@ Program compile_circuit(const std::string &main_name, const std::vector<Fr> &par
         return P;
     }
     P.codes.insert(P.codes.end(), B.flat, B.flat + B.flat_n);
-    uint32_t tile_signals = TILE_SIGNALS;
+    uint32_t tile_signals = LAYOUT_TILE_SIGNALS;
 #ifdef POB_TUNING
     if (const char *v = getenv("POB_TILE_SIGNALS")) { uint32_t t = (uint32_t)atoi(v); if (t >= 128 && t <= TILE_SIGNALS && t % 128 == 0) tile_signals = t; }   // 128: the TMA copy of a tile's descriptors needs 16-byte alignment
 #endif

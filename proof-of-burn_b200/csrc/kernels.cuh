@@ -364,8 +364,8 @@ struct ExpandArgs {
 };
 
 // k_expand_round: grid = (KeccakfRound tiles, instances in the group) -- 95.8 % of the witness.  One CTA streams one
-// tile (<= 8192 entries = 256 KiB) with one 128-bit store per half entry.  The source of every entry follows from an 8-byte
-// descriptor per 64 entries and a lane word of the round; the tile's <= 130 descriptors and the round's 263 words are
+// tile (<= 4096 entries = 128 KiB in the O0 layout) with one 128-bit store per half entry.  The source of every entry
+// follows from an 8-byte descriptor per 64 entries and a lane word of the round; the tile's <= 130 descriptors and the round's 263 words are
 // staged in shared memory by two TMA bulk copies, so the streaming loop touches no global memory but the witness itself.
 template <int T>
 __global__ void __launch_bounds__(T) k_expand_round(const ExpandArgs a) {

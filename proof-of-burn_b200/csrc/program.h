@@ -122,6 +122,9 @@ struct Level { uint32_t t_begin, t_end, w_begin, w_end, p_begin, p_end, s_begin,
 // ---- expand tiles: a contiguous run of witness entries and where its codes live -------------------------------
 struct Tile { uint64_t dst; uint32_t n, code_off, ubase, pad; };  // BIT codes are relative to ubase; pad = 1: round tile (all BIT)
 static const uint32_t TILE_SIGNALS = 8192;
+// entries per tile of the O0 layout (128 KiB of witness).  Resident k_expand_round CTAs write neighbouring tiles, so smaller
+// tiles keep the write front narrower: 4096 made the round tiles 4 % faster than 8192 on compressible slots (DESIGN.md §2.3)
+static const uint32_t LAYOUT_TILE_SIGNALS = 4096;
 static const uint32_t MAX_TILE_SIGNALS = 32768;  // upper bound for the POB_TILE_SIGNALS tuning knob
 
 // ---- constraint system of the circuit (SURVEY.md 8(f) rank 4: on-GPU self-check; rank 2: reduced witness map) -------
