@@ -208,6 +208,40 @@ int pob_selfcheck(pob_handle *h, uint32_t index, pob_check_report *out);
 /* host-only: compile the constraint system of a circuit shape and report its size (no GPU needed) */
 int pob_constraint_info(const char *main_name, const uint64_t *params, int nparams, int hcreate, pob_check_report *out);
 
+/* ---- the circuit as an R1CS: the `.r1cs` a prover is set up from, and its rows on the GPU ---------------------------------
+ * replaces: the `.r1cs` of `circom --r1cs`.  The rows are the constraint system above in record order -- flat eq, kc, r1 records,
+ * then those of the shared KeccakfRound set for every round block -- without the hint records (not constraints of the circuit)
+ * and without records whose A, B and C are all empty after merging (the `witness[0] == 1` record).  eq (a, b) is the row
+ * 0 * 0 = w[a] - w[b], kc (a, k) is 0 * 0 = w[a] - k w0, an A*B = C record keeps its combinations (B empty when A is); inside a
+ * combination terms are merged by wire, zero coefficients dropped, wires ascending.  With POB_CREATE_O1 the wires are the
+ * reduced witness entries: every term moves to its equality class's representative or, in a constant class, to wire 0 times the
+ * constant; the eq / kc rows vanish, except one row `s - representative` (or `s - k w0`) for each main input / output that is not
+ * its class's representative.  The file and the reduced witness agree on the wire order by construction, whatever order circom
+ * itself would choose.  n_wires..n_labels are the header fields of the file. */
+typedef struct {
+    uint64_t n_wires;          /* == pob_desc.n_signals for the same flags */
+    uint32_t n_pub_out;        /* n_outputs */
+    uint32_t n_pub_in;         /* 0: no main declares public inputs */
+    uint32_t n_prv_in;         /* n_inputs */
+    uint64_t n_labels;         /* n_signals_o0 (section 3 maps wire -> --O0 signal id: identity for --O0, pob_witness_map for O1) */
+    uint64_t n_constraints;    /* rows (mConstraints) */
+    uint64_t n_nonlinear;      /* rows with a non-empty A */
+    uint64_t n_terms;          /* A + B + C terms over all rows */
+    uint64_t file_bytes;       /* size of the .r1cs */
+} pob_r1cs_desc;
+/* host-only: write the iden3 binary `.r1cs` (version 1; coefficients canonical 32-byte LE, as circom writes them) of a circuit
+ * shape; hcreate as in pob_layout_info (bit 0, POB_CREATE_O1).  The file is streamed, never held in memory (a main-shape --O0
+ * file is tens of GB).  path == NULL: count only, write nothing.  A failed open or short write is POB_E_IO. */
+int pob_write_r1cs(const char *main_name, const uint64_t *params, int nparams, int hcreate, const char *path, pob_r1cs_desc *out);
+/* every .r1cs row of the handle's form (O0 or O1) against resident witness `index`; record ids in the report are row indices;
+ * n_hints / n_hint_failed are 0, signals_read = wires referenced.  The first call builds and uploads the row plan. */
+int pob_r1cs_check(pob_handle *h, uint32_t index, pob_check_report *out);
+/* the first stage of a GPU Groth16 prover: rows [first_row, first_row + n_rows) of the .r1cs, a[k], b[k], c[k] = A.w, B.w, C.w of
+ * row first_row + k as 32-byte canonical LE field elements, into caller device buffers (any may be NULL: not computed).
+ * consumer_stream NULL: returns when done; else (a cudaStream_t) enqueued on that stream, which the caller has ordered after the
+ * witness (pob_acquire on it, or a finished pob_run_batch).  first_row + n_rows beyond the row count: POB_E_RANGE. */
+int pob_r1cs_products(pob_handle *h, uint32_t index, uint64_t first_row, uint64_t n_rows, void *a, void *b, void *c, void *consumer_stream);
+
 /* ---- the step just before the path (SURVEY.md 8(f) rank 3) ------------------------------------------------------
  * replaces: find_burn_key() of the reference input generator (tests/main.py:47-56): starting at start_key, find the
  * first burnKey >= start_key whose keccak256(burnKey[32 BE] | revealAmount[32 BE] | burnExtraCommitment[32 BE] |

@@ -18,6 +18,7 @@
 #include <stdexcept>
 #include <unordered_map>
 #include "poseidon_constants_data.h"
+#include "r1cs.h"
 #include "vm_exec.h"
 
 namespace pob {
@@ -2040,6 +2041,34 @@ struct Reduction { std::vector<uint32_t> round_keep; std::vector<uint8_t> keep_f
 static uint32_t uf_find(std::vector<uint32_t> &p, uint32_t x) { while (p[x] != x) { p[x] = p[p[x]]; x = p[x]; } return x; }
 static void uf_union(std::vector<uint32_t> &p, uint32_t a, uint32_t b) { a = uf_find(p, a); b = uf_find(p, b); if (a == b) return; if (a < b) p[b] = a; else p[a] = b; }
 
+// equality classes of the N --O0 signals under the eq records of a compiled constraint system (the representative of a class is its
+// lowest-numbered member), and which classes are constant (a member has a kc record; witness[0]'s class always is)
+struct EqClasses {
+    std::vector<uint32_t> parent; std::vector<uint8_t> is_const_root;
+    uint32_t root(uint32_t s) { return uf_find(parent, s); }
+};
+static EqClasses eq_classes(const Program &P, uint64_t N) {
+    EqClasses E;
+    std::vector<uint32_t> &parent = E.parent; std::vector<uint8_t> &is_const_root = E.is_const_root;
+    // the shared round set, resolved once: relative representative (lowest index) and constness per relative signal
+    std::vector<uint32_t> rp(ROUND_SIGNALS); for (uint32_t i = 0; i < ROUND_SIGNALS; i++) rp[i] = i;
+    for (size_t i = 0; i + 1 < P.cons_round.eq.size(); i += 2) uf_union(rp, P.cons_round.eq[i], P.cons_round.eq[i + 1]);
+    std::vector<uint8_t> rconst(ROUND_SIGNALS, 0);
+    for (const ConsTerm &t : P.cons_round.kc) rconst[uf_find(rp, t.idx)] = 1;
+    parent.resize(N); is_const_root.assign(N, 0);
+    for (uint64_t i = 0; i < N; i++) parent[i] = (uint32_t)i;
+    for (uint64_t base : P.round_block_sig) for (uint32_t i = 0; i < ROUND_SIGNALS; i++) { const uint32_t r = uf_find(rp, i); parent[base + i] = (uint32_t)(base + r); if (r == i && rconst[i]) is_const_root[base + i] = 1; }
+    for (size_t i = 0; i + 1 < P.cons_flat.eq.size(); i += 2) {
+        uint32_t a = uf_find(parent, P.cons_flat.eq[i]), b2 = uf_find(parent, P.cons_flat.eq[i + 1]);
+        if (a == b2) continue;
+        const uint8_t c = is_const_root[a] | is_const_root[b2];
+        if (a < b2) { parent[b2] = a; is_const_root[a] = c; } else { parent[a] = b2; is_const_root[b2] = c; }
+    }
+    for (const ConsTerm &t : P.cons_flat.kc) is_const_root[uf_find(parent, t.idx)] = 1;
+    is_const_root[uf_find(parent, 0)] = 1;                                    // witness[0] itself is kept as main I/O
+    return E;
+}
+
 Program compile_circuit(const std::string &main_name, const std::vector<Fr> &params, bool hcreate, bool want_constraints, int opt_level) {
     if (opt_level < 0 || opt_level > 1) throw std::runtime_error("pob: opt_level must be 0 (--O0) or 1 (signal=signal / signal=constant elimination)");
     const bool user_wants_constraints = want_constraints;
@@ -2185,28 +2214,11 @@ Program compile_circuit(const std::string &main_name, const std::vector<Fr> &par
     }
     // ---- reduced witness: which signals stay ----
     std::vector<uint32_t> round_keep;            // retained relative indices inside a KeccakfRound block (same for every block)
-    std::vector<uint32_t> parent;                // union-find over all --O0 signals
-    std::vector<uint8_t> is_const_root;
     if (opt_level) {
         const uint64_t N = B.nsig;
-        // the shared round set, resolved once: relative representative (lowest index) and constness per relative signal
-        std::vector<uint32_t> rp(ROUND_SIGNALS); for (uint32_t i = 0; i < ROUND_SIGNALS; i++) rp[i] = i;
-        for (size_t i = 0; i + 1 < P.cons_round.eq.size(); i += 2) uf_union(rp, P.cons_round.eq[i], P.cons_round.eq[i + 1]);
-        std::vector<uint8_t> rconst(ROUND_SIGNALS, 0);
-        for (const ConsTerm &t : P.cons_round.kc) rconst[uf_find(rp, t.idx)] = 1;
-        parent.resize(N); is_const_root.assign(N, 0);
-        for (uint64_t i = 0; i < N; i++) parent[i] = (uint32_t)i;
-        for (uint64_t base : B.round_sigs) for (uint32_t i = 0; i < ROUND_SIGNALS; i++) { const uint32_t r = uf_find(rp, i); parent[base + i] = (uint32_t)(base + r); if (r == i && rconst[i]) is_const_root[base + i] = 1; }
-        for (size_t i = 0; i + 1 < P.cons_flat.eq.size(); i += 2) {
-            uint32_t a = uf_find(parent, P.cons_flat.eq[i]), b2 = uf_find(parent, P.cons_flat.eq[i + 1]);
-            if (a == b2) continue;
-            const uint8_t c = is_const_root[a] | is_const_root[b2];
-            if (a < b2) { parent[b2] = a; is_const_root[a] = c; } else { parent[a] = b2; is_const_root[b2] = c; }
-        }
-        for (const ConsTerm &t : P.cons_flat.kc) is_const_root[uf_find(parent, t.idx)] = 1;
+        EqClasses E = eq_classes(P, N);
         const uint64_t n_io = 1ull + n_out + n_in;
-        is_const_root[uf_find(parent, 0)] = 1;                                    // witness[0] itself is kept as main I/O
-        auto kept = [&](uint64_t s) { if (s < n_io) return true; const uint32_t r = uf_find(parent, (uint32_t)s); return r == s && !is_const_root[r]; };
+        auto kept = [&](uint64_t s) { if (s < n_io) return true; const uint32_t r = E.root((uint32_t)s); return r == s && !E.is_const_root[r]; };
         // inside a round block the retained set must be the same for all blocks (it is: in/out tie to the enclosing Keccakf's
         // lower-numbered midRound signals, everything else is block-internal); verified below while the map is built
         if (!B.round_sigs.empty()) { const uint64_t b0 = B.round_sigs[0]; for (uint32_t i = 0; i < ROUND_SIGNALS; i++) if (kept(b0 + i)) round_keep.push_back(i); }
@@ -2282,6 +2294,157 @@ Program compile_circuit(const std::string &main_name, const std::vector<Fr> &par
     // stream costs DRAM efficiency, so all round tiles go first, the rest last.
     std::stable_sort(P.tiles.begin(), P.tiles.end(), [](const Tile &a, const Tile &b) { return a.pad > b.pad; });
     return P;
+}
+
+// ---- the .r1cs row plan (r1cs.h) -----------------------------------------------------------------------------------------
+// A combination as (sort key, coefficient): key = wire, except in the block-relative round set, where CONS_ONE (wire 0) is key 0
+// and relative signal i is key i + 1, so that ascending keys are ascending absolute wires in every block.
+static uint64_t lc_key(uint32_t idx, bool rel) { return idx == CONS_ONE ? 0 : rel ? (uint64_t)idx + 1 : idx; }
+static uint64_t lc_idx(uint64_t key, bool rel) { return !rel ? key : key == 0 ? CONS_ONE : key - 1; }
+static LC lc_of(const ConsTerm *t, uint32_t n, const std::vector<Fr> &konst, bool rel) {
+    LC L; for (uint32_t i = 0; i < n; i++) L.sf(lc_key(t[i].idx, rel), cons_coef_value(t[i].coef, konst.data(), 0)); return L;
+}
+// merge by key, drop zero coefficients, sort ascending
+static void lc_normalize(LC &L) {
+    std::sort(L.t.begin(), L.t.end(), [](const std::pair<uint64_t, Fr> &x, const std::pair<uint64_t, Fr> &y) { return x.first < y.first; });
+    size_t o = 0;
+    for (size_t i = 0; i < L.t.size();) {
+        std::pair<uint64_t, Fr> m = L.t[i++];
+        while (i < L.t.size() && L.t[i].first == m.first) m.second = fr_add(m.second, L.t[i++].second);
+        if (!fr_is_zero(m.second)) L.t[o++] = m;
+    }
+    L.t.resize(o);
+}
+static void lc_unkey(LC &L, bool rel) { for (auto &q : L.t) q.first = lc_idx(q.first, rel); }
+// one r1 row of the plan: normalised, B emptied when A is, left out when A and C are empty (returns false then)
+static bool plan_r1(ConsSink &S, LC &A, LC &Bq, LC &C, bool rel) {
+    lc_normalize(A); lc_normalize(Bq); lc_normalize(C);
+    if (A.t.empty()) Bq.t.clear();
+    if (A.t.empty() && C.t.empty()) return false;
+    lc_unkey(A, rel); lc_unkey(Bq, rel); lc_unkey(C, rel);
+    S.r1(A, Bq, C);
+    return true;
+}
+
+// --O0 rows of one ConsSet: eq with a == b, kc `w0 == 1` and all-empty r1 records dropped, hints dropped, r1 combinations normalised
+static void plan_o0_set(const ConsSet &in, ConsSink &S, bool rel) {
+    const std::vector<Fr> &konst = *S.konst;
+    for (size_t i = 0; i + 1 < in.eq.size(); i += 2) if (in.eq[i] != in.eq[i + 1]) S.eq(in.eq[i], in.eq[i + 1]);
+    for (const ConsTerm &t : in.kc) {
+        const bool on_one = t.idx == CONS_ONE || (!rel && t.idx == 0);
+        if (on_one && cc_kind(t.coef) != CC_RCBIT && fr_eq(cons_coef_value(t.coef, konst.data(), 0), fr_from_u64(1))) continue;   // 1 w0 - 1 w0
+        S.kc_raw(t.idx, t.coef);
+    }
+    for (const ConsR1 &r : in.r1) {
+        if (r1_hint(r)) continue;
+        const ConsTerm *t = in.terms.data() + r.off;
+        LC A = lc_of(t, r.na, konst, rel), Bq = lc_of(t + r.na, r.nb, konst, rel), C = lc_of(t + r.na + r.nb, r1_nc(r), konst, rel);
+        plan_r1(S, A, Bq, C, rel);
+    }
+}
+
+// terms of the rows of one set in block round r (kc rows: C = w[a] - k w0 has 1 or 2 terms; eq rows 2)
+static uint64_t plan_set_terms(const ConsSet &S, const std::vector<Fr> &konst, bool rel, uint64_t rc) {
+    uint64_t n = S.eq.size();
+    for (const ConsTerm &t : S.kc) {
+        const bool on_one = t.idx == CONS_ONE || (!rel && t.idx == 0);
+        n += (on_one || fr_is_zero(cons_coef_value(t.coef, konst.data(), rc))) ? 1 : 2;
+    }
+    for (const ConsR1 &r : S.r1) n += r.na + r.nb + r1_nc(r);
+    return n;
+}
+
+RowPlan build_row_plan(const std::string &main_name, const std::vector<Fr> &params, bool hcreate, int opt_level) {
+    Program P = compile_circuit(main_name, params, hcreate, true, opt_level);
+    RowPlan R;
+    R.opt_level = opt_level; R.n_wires = P.n_signals; R.n_labels = P.n_signals_o0; R.n_outputs = P.n_outputs; R.n_inputs = P.n_inputs;
+    R.konst = P.cons_konst;
+    std::unordered_map<std::array<uint32_t, 8>, uint32_t, FrHash> kix;         // the emitter's constant dedupe, seeded with its table
+    for (size_t i = 0; i < R.konst.size(); i++) { std::array<uint32_t, 8> key; memcpy(key.data(), R.konst[i].l, 32); kix.emplace(key, (uint32_t)i); }
+    ConsSink fs; fs.S = &R.flat; fs.konst = &R.konst; fs.kix = &kix;
+    if (!opt_level) {
+        ConsSink rs; rs.S = &R.round; rs.konst = &R.konst; rs.kix = &kix;
+        plan_o0_set(P.cons_flat, fs, false);
+        plan_o0_set(P.cons_round, rs, true);
+        R.bases = P.round_block_sig;
+        R.n_terms = plan_set_terms(R.flat, R.konst, false, 0);
+        uint64_t per_round[24];
+        for (int r = 0; r < 24; r++) per_round[r] = plan_set_terms(R.round, R.konst, true, keccak_rc(r));
+        for (size_t b = 0; b < R.bases.size(); b++) R.n_terms += per_round[b % 24];
+        uint64_t nl_flat = 0, nl_round = 0;
+        for (const ConsR1 &r : R.flat.r1) nl_flat += r.na != 0;
+        for (const ConsR1 &r : R.round.r1) nl_round += r.na != 0;
+        R.n_nonlinear = nl_flat + R.bases.size() * nl_round;
+        return R;
+    }
+    // --O1: substitute the equality classes of the reduction into the --O0 rows, in the same order.  A term on a signal moves to its
+    // class representative (kept, so it has a reduced wire) or, in a constant class, becomes coef * value on wire 0; eq and kc
+    // records thereby become empty.  A main input / output that is not its class's representative keeps one row, s - rep (or
+    // s - k w0), at its first eq / kc record, so that its own wire stays constrained.
+    const uint64_t N = P.n_signals_o0, n_io = 1ull + P.n_outputs + P.n_inputs;
+    EqClasses E = eq_classes(P, N);
+    std::vector<uint32_t> red(N, NONE_IDX);
+    for (size_t k = 0; k < P.witness_map.size(); k++) red[P.witness_map[k]] = (uint32_t)k;
+    std::unordered_map<uint32_t, Fr> cval;                                     // value of every constant class, by representative
+    auto set_val = [&](uint32_t s, const Fr &v) {
+        const uint32_t r = E.root(s);
+        auto it = cval.find(r);
+        if (it == cval.end()) cval.emplace(r, v);
+        else if (!fr_eq(it->second, v)) throw std::runtime_error("pob: internal: two constants disagree in one equality class (signal " + std::to_string(s) + ")");
+    };
+    set_val(0, fr_from_u64(1));
+    for (const ConsTerm &t : P.cons_flat.kc) set_val(t.idx, cons_coef_value(t.coef, P.cons_konst.data(), 0));
+    for (size_t b = 0; b < P.round_block_sig.size(); b++)
+        for (const ConsTerm &t : P.cons_round.kc) set_val((uint32_t)(P.round_block_sig[b] + t.idx), cons_coef_value(t.coef, P.cons_konst.data(), keccak_rc((int)(b % 24))));
+    auto subst = [&](LC &L, uint32_t s, const Fr &c) {
+        const uint32_t r = E.root(s);
+        if (E.is_const_root[r]) {
+            auto it = cval.find(r);
+            if (it == cval.end()) throw std::runtime_error("pob: internal: constant class without a value");
+            L.sf(0, fr_mul(c, it->second));
+        } else {
+            if (red[r] == NONE_IDX) throw std::runtime_error("pob: internal: class representative is not a reduced-witness entry");
+            L.sf(red[r], c);
+        }
+    };
+    auto subst_lc = [&](const ConsTerm *t, uint32_t n, uint64_t base) {
+        LC L;
+        for (uint32_t i = 0; i < n; i++) {
+            const Fr c = cons_coef_value(t[i].coef, P.cons_konst.data(), 0);
+            if (t[i].idx == CONS_ONE) L.sf(0, c); else subst(L, (uint32_t)(base + t[i].idx), c);
+        }
+        return L;
+    };
+    std::vector<uint8_t> io_done(n_io, 0);
+    auto io_row = [&](uint32_t s) {
+        if (s == 0 || s >= n_io || io_done[s]) return;
+        io_done[s] = 1;
+        const uint32_t r = E.root(s);
+        if (r == s && !E.is_const_root[r]) return;                              // its own representative: terms already land on it
+        LC A, Bq, C; C.sf(red[s], fr_from_u64(1)); subst(C, s, fr_neg(fr_from_u64(1)));
+        plan_r1(fs, A, Bq, C, false);
+    };
+    for (size_t i = 0; i + 1 < P.cons_flat.eq.size(); i += 2) { io_row(P.cons_flat.eq[i]); io_row(P.cons_flat.eq[i + 1]); }
+    for (const ConsTerm &t : P.cons_flat.kc) io_row(t.idx);
+    auto r1_rows = [&](const ConsSet &S, uint64_t base) {
+        for (const ConsR1 &r : S.r1) {
+            if (r1_hint(r)) continue;
+            const ConsTerm *t = S.terms.data() + r.off;
+            LC A = subst_lc(t, r.na, base), Bq = subst_lc(t + r.na, r.nb, base), C = subst_lc(t + r.na + r.nb, r1_nc(r), base);
+            plan_r1(fs, A, Bq, C, false);
+        }
+    };
+    r1_rows(P.cons_flat, 0);
+    for (uint64_t base : P.round_block_sig) r1_rows(P.cons_round, base);
+    R.witness_map = std::move(P.witness_map);
+    R.n_terms = plan_set_terms(R.flat, R.konst, false, 0);
+    for (const ConsR1 &r : R.flat.r1) R.n_nonlinear += r.na != 0;
+    return R;
+}
+
+uint64_t RowPlan::file_bytes() const {
+    // magic, version, nSections; 3 section headers; header content; per row 3 term counts, per term wire + coefficient; labels
+    return 12 + 3 * 12 + 64 + 12 * n_rows() + 36 * n_terms + 8 * n_wires;
 }
 
 // Component list of a circuit shape in numbering order: one line `first_signal,n_own_signals,template` per component instance

@@ -19,6 +19,7 @@
 //             (cp.async.bulk + mbarrier).
 //   k_check_eq / k_check_kc / k_check_r1  every constraint of the circuit evaluated against a resident witness (cons_check.h).
 //   k_check_rounds  layout-independent check of every KeccakfRound block (textbook round on its in/out signals).
+//   k_r1cs_products  A.w, B.w, C.w of a window of `.r1cs` rows (r1cs.h row plan) against a resident witness, for a GPU prover.
 //   k_digest  64-bit digest of a materialised witness (parity tests at full size; the built-in on-GPU consumer).
 //   k_pow_grind  proof-of-work burn-key search (the step before the path): one candidate key per thread.
 #pragma once
@@ -585,6 +586,47 @@ __global__ void __launch_bounds__(256) k_check_r1(const CheckArgs a) {
         const uint64_t blk = t / per, r = t - blk * per, base = a.bases ? a.bases[blk] : 0;
         const ConsR1 rec = a.V.r1[r];
         if (!cons_r1_ok(a.wit, base, rec, a.V.terms, a.konst)) check_fail(a, a.id0 + blk * a.V.n_records() + a.V.n_eq + a.V.n_kc + r, r1_hint(rec));
+    }
+}
+
+// ---- .r1cs row products (r1cs.h): out[k] = A.w, B.w, C.w of row first + k, 32-byte canonical little-endian ------------------
+// Row k of the plan is decoded into (set, block, kind, local record): the flat set's eq / kc / r1 records first, then the round
+// set once per block.  A LANE PAIR owns a row: both lanes evaluate it (the same loads, merged in the warp's request) and lane h
+// stores 16-byte half h of each product, so that a warp's store covers 16 rows = 512 contiguous bytes per vector -- one thread
+// writing a whole 32-byte entry as two 128-bit stores is the pattern that halved the expand kernels' rate (DESIGN.md §2.3).
+struct R1csArgs {
+    ConsView flat, round; const Fr *konst; const uint64_t *wit;
+    const uint64_t *bases;                          // first witness index of every round block (n_blocks of them)
+    uint64_t first, n;                              // rows [first, first + n)
+    uint4 *a, *b, *c;                               // n entries each, or null (not computed)
+};
+__device__ __forceinline__ void st_half(uint4 *out, uint64_t k, uint32_t h, const Fr &v) {
+    out[2 * k + h] = h ? make_uint4(v.l[4], v.l[5], v.l[6], v.l[7]) : make_uint4(v.l[0], v.l[1], v.l[2], v.l[3]);   // no dynamic index: Fr stays in registers
+}
+__global__ void __launch_bounds__(256) k_r1cs_products(const R1csArgs a) {
+    const uint32_t h = threadIdx.x & 1u;
+    const uint64_t nf = a.flat.n_records(), per = a.round.n_records();
+    const bool want_ab = a.a || a.b;
+    for (uint64_t k = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 1; k < a.n; k += ((uint64_t)gridDim.x * blockDim.x) >> 1) {
+        uint64_t r = a.first + k, base = 0, rc = 0;
+        const bool in_round = r >= nf;
+        if (in_round) { const uint64_t q = r - nf, blk = q / per; r = q - blk * per; base = a.bases[blk]; rc = c_keccak_rc[blk % 24]; }
+        const ConsView V = in_round ? a.round : a.flat;
+        Fr A = fr_zero(), B = fr_zero(), C;
+        if (r < V.n_eq) {                                                   // C = w[a] - w[b]
+            C = fr_sub(cons_load(a.wit, base, V.eq[2 * r]), cons_load(a.wit, base, V.eq[2 * r + 1]));
+        } else if (r < V.n_eq + V.n_kc) {                                   // C = w[a] - k w0
+            const ConsTerm t = V.kc[r - V.n_eq];
+            C = fr_sub(cons_load(a.wit, base, t.idx), cons_coef_value(t.coef, a.konst, rc));
+        } else {
+            const ConsR1 rec = V.r1[r - V.n_eq - V.n_kc];
+            const ConsTerm *t = V.terms + rec.off;
+            C = a.c ? cons_lc(a.wit, base, t + rec.na + rec.nb, r1_nc(rec), a.konst) : fr_zero();
+            if (want_ab && rec.na) { A = cons_lc(a.wit, base, t, rec.na, a.konst); B = cons_lc(a.wit, base, t + rec.na, rec.nb, a.konst); }
+        }
+        if (a.a) st_half(a.a, k, h, A);
+        if (a.b) st_half(a.b, k, h, B);
+        if (a.c) st_half(a.c, k, h, C);
     }
 }
 

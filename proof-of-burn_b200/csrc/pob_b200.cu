@@ -27,6 +27,7 @@
 #include "../../include/pob_b200.h"
 #include "compiler.h"
 #include "kernels.cuh"
+#include "r1cs.h"
 
 using namespace pob;
 
@@ -222,11 +223,11 @@ struct pob_handle {
     } B;
     Exporter *exporter = nullptr;
     pob_timing timing{};
-    // constraint system for pob_selfcheck, built on first use
+    // constraint system for pob_selfcheck, and the .r1cs row plan for pob_r1cs_check / pob_r1cs_products, each built on first use
     struct DevCons {
         bool ready = false; ConsView flat{}, round{}; Fr *konst = nullptr; uint64_t *bases = nullptr; uint32_t n_blocks = 0;
         unsigned long long *rep = nullptr; std::vector<void *> allocs; pob_check_report info{};
-    } cons;
+    } cons, r1cs;
 };
 
 static void cons_info(const Program &P, pob_check_report *r) {
@@ -248,9 +249,9 @@ static void cons_info(const Program &P, pob_check_report *r) {
     for (uint8_t v : seen) r->signals_read += v;
     r->first_failed = ~0ull;
 }
-static ConsView upload_cons(pob_handle *h, const ConsSet &S) {
+static ConsView upload_cons(pob_handle::DevCons &C, const ConsSet &S) {
     ConsView v{};
-    auto up = [&](const void *src, size_t bytes) { void *d = nullptr; CU(cudaMalloc(&d, std::max<size_t>(16, bytes))); if (bytes) CU(cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice)); h->cons.allocs.push_back(d); return d; };
+    auto up = [&](const void *src, size_t bytes) { void *d = nullptr; CU(cudaMalloc(&d, std::max<size_t>(16, bytes))); if (bytes) CU(cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice)); C.allocs.push_back(d); return d; };
     v.eq = (const uint32_t *)up(S.eq.data(), S.eq.size() * 4); v.n_eq = S.eq.size() / 2;
     v.kc = (const ConsTerm *)up(S.kc.data(), S.kc.size() * sizeof(ConsTerm)); v.n_kc = S.kc.size();
     v.r1 = (const ConsR1 *)up(S.r1.data(), S.r1.size() * sizeof(ConsR1)); v.n_r1 = S.r1.size();
@@ -545,11 +546,25 @@ int pob_write_components(const char *main_name, const uint64_t *params, int npar
     return POB_OK;
 }
 
+int pob_write_r1cs(const char *main_name, const uint64_t *params, int nparams, int hcreate, const char *path, pob_r1cs_desc *out) {
+    if (!main_name || !out || (nparams > 0 && !params)) return fail(POB_E_BAD_ARG, "pob_write_r1cs: null argument");
+    try {
+        const RowPlan R = build_row_plan(main_name, params_vec(params, nparams), flag_hcreate(hcreate), flag_opt(hcreate));
+        memset(out, 0, sizeof *out);
+        out->n_wires = R.n_wires; out->n_pub_out = R.n_outputs; out->n_pub_in = 0; out->n_prv_in = R.n_inputs; out->n_labels = R.n_labels;
+        out->n_constraints = R.n_rows(); out->n_nonlinear = R.n_nonlinear; out->n_terms = R.n_terms; out->file_bytes = R.file_bytes();
+        if (path) write_r1cs(R, path);
+    } catch (const R1csIoError &e) { return fail(POB_E_IO, std::string("pob_write_r1cs: ") + e.what()); }
+    catch (const std::exception &e) { return fail(POB_E_COMPILE, e.what()); }
+    return POB_OK;
+}
+
 void pob_destroy(pob_handle *h) {
     if (!h) return;
     cudaSetDevice(h->device);
     delete h->exporter; h->exporter = nullptr;
     for (void *p : h->cons.allocs) cudaFree(p);
+    for (void *p : h->r1cs.allocs) cudaFree(p);
     if (h->s_eval) cudaStreamSynchronize(h->s_eval);
     if (h->s_exp2) cudaStreamSynchronize(h->s_exp2);
     if (h->s_exp) cudaStreamSynchronize(h->s_exp);
@@ -934,6 +949,34 @@ int pob_constraint_info(const char *main_name, const uint64_t *params, int npara
     return POB_OK;
 }
 
+// every record of a device constraint set (flat set, then the round set once per block) against witness slot s; record ids are
+// positions in that order
+static void check_sets(pob_handle *h, pob_handle::DevCons &C, const uint64_t *s, pob_check_report *out) {
+    const unsigned long long init[3] = {0, 0, ~0ull};
+    CU(cudaMemcpy(C.rep, init, 24, cudaMemcpyHostToDevice));
+    cudaEvent_t e0, e1; CU(cudaEventCreate(&e0)); CU(cudaEventCreate(&e1));
+    CU(cudaEventRecord(e0, 0));
+    auto grid = [h](uint64_t n) { return (unsigned)std::min<uint64_t>((n + 255) / 256, h->n_sms * 64ull); };
+    CheckArgs fa{C.flat, C.konst, s, nullptr, 0, 0, C.rep};
+    if (C.flat.n_eq) k_check_eq<<<grid(C.flat.n_eq), 256>>>(fa);
+    if (C.flat.n_kc) k_check_kc<<<grid(C.flat.n_kc), 256>>>(fa);
+    if (C.flat.n_r1) k_check_r1<<<grid(C.flat.n_r1), 256>>>(fa);
+    if (C.n_blocks) {
+        CheckArgs ra{C.round, C.konst, s, C.bases, C.n_blocks, C.flat.n_records(), C.rep};
+        if (C.round.n_eq) k_check_eq<<<grid(C.round.n_eq * C.n_blocks), 256>>>(ra);
+        if (C.round.n_kc) k_check_kc<<<grid(C.round.n_kc * C.n_blocks), 256>>>(ra);
+        if (C.round.n_r1) k_check_r1<<<grid(C.round.n_r1 * C.n_blocks), 256>>>(ra);
+    }
+    CU(cudaEventRecord(e1, 0));
+    CU(cudaGetLastError());
+    unsigned long long rep[3];
+    CU(cudaMemcpy(rep, C.rep, 24, cudaMemcpyDeviceToHost));
+    *out = C.info;
+    CU(cudaEventElapsedTime(&out->ms, e0, e1));
+    cudaEventDestroy(e0); cudaEventDestroy(e1);
+    out->n_failed = rep[0]; out->n_hint_failed = rep[1]; out->first_failed = rep[2];
+}
+
 int pob_selfcheck(pob_handle *h, uint32_t index, pob_check_report *out) {
     if (!h || !out) return fail(POB_E_BAD_ARG, "pob_selfcheck: null argument");
     if (h->P.opt_level) return fail(POB_E_BAD_ARG, "pob_selfcheck: the constraint system is stated over the --O0 witness; create the handle without POB_CREATE_O1");
@@ -945,35 +988,13 @@ int pob_selfcheck(pob_handle *h, uint32_t index, pob_check_report *out) {
             Program Q = compile_circuit(h->P.main_name, h->P.params, h->P.hcreate, true);
             if (Q.n_signals != h->P.n_signals) throw std::runtime_error("internal: constraint compile disagrees on the witness size");
             cons_info(Q, &C.info);
-            C.flat = upload_cons(h, Q.cons_flat); C.round = upload_cons(h, Q.cons_round);
+            C.flat = upload_cons(C, Q.cons_flat); C.round = upload_cons(C, Q.cons_round);
             C.konst = upload(Q.cons_konst); C.allocs.push_back(C.konst);
             C.bases = upload(Q.round_block_sig); C.allocs.push_back(C.bases); C.n_blocks = (uint32_t)Q.round_block_sig.size();
             CU(cudaMalloc(&C.rep, 24)); C.allocs.push_back(C.rep);
             C.ready = true;
         }
-        const unsigned long long init[3] = {0, 0, ~0ull};
-        CU(cudaMemcpy(C.rep, init, 24, cudaMemcpyHostToDevice));
-        cudaEvent_t e0, e1; CU(cudaEventCreate(&e0)); CU(cudaEventCreate(&e1));
-        CU(cudaEventRecord(e0, 0));
-        auto grid = [h](uint64_t n) { return (unsigned)std::min<uint64_t>((n + 255) / 256, h->n_sms * 64ull); };
-        CheckArgs fa{C.flat, C.konst, s, nullptr, 0, 0, C.rep};
-        if (C.flat.n_eq) k_check_eq<<<grid(C.flat.n_eq), 256>>>(fa);
-        if (C.flat.n_kc) k_check_kc<<<grid(C.flat.n_kc), 256>>>(fa);
-        if (C.flat.n_r1) k_check_r1<<<grid(C.flat.n_r1), 256>>>(fa);
-        if (C.n_blocks) {
-            CheckArgs ra{C.round, C.konst, s, C.bases, C.n_blocks, C.flat.n_records(), C.rep};
-            k_check_eq<<<grid(C.round.n_eq * C.n_blocks), 256>>>(ra);
-            k_check_kc<<<grid(C.round.n_kc * C.n_blocks), 256>>>(ra);
-            k_check_r1<<<grid(C.round.n_r1 * C.n_blocks), 256>>>(ra);
-        }
-        CU(cudaEventRecord(e1, 0));
-        CU(cudaGetLastError());
-        unsigned long long rep[3];
-        CU(cudaMemcpy(rep, C.rep, 24, cudaMemcpyDeviceToHost));
-        *out = C.info;
-        CU(cudaEventElapsedTime(&out->ms, e0, e1));
-        cudaEventDestroy(e0); cudaEventDestroy(e1);
-        out->n_failed = rep[0]; out->n_hint_failed = rep[1]; out->first_failed = rep[2];
+        check_sets(h, C, s, out);
     } catch (const std::exception &e) { return fail(POB_E_CUDA, std::string("pob_selfcheck: ") + e.what()); }
     return POB_OK;
 }
@@ -1007,6 +1028,62 @@ int pob_write_wtns(pob_handle *h, uint32_t index, const char *path) {
         h->exporter->drain();
         if (h->exporter->io_err) return fail(POB_E_IO, std::string("short write to ") + path);
     } catch (const std::exception &e) { return fail(POB_E_CUDA, std::string("pob_write_wtns: ") + e.what()); }
+    return POB_OK;
+}
+
+// ---- the .r1cs rows on the GPU -------------------------------------------------------------------------------------
+// the handle's row plan (r1cs.h, same form as the handle's witness) in device memory, built and uploaded on first use
+static pob_handle::DevCons &ensure_r1cs(pob_handle *h) {
+    pob_handle::DevCons &C = h->r1cs;
+    if (C.ready) return C;
+    const RowPlan R = build_row_plan(h->P.main_name, h->P.params, h->P.hcreate, h->P.opt_level);
+    if (R.n_wires != h->P.n_signals) throw std::runtime_error("internal: the row plan disagrees on the witness size");
+    pob_check_report &I = C.info;
+    memset(&I, 0, sizeof I);
+    I.n_constraints = R.n_rows(); I.n_nonlinear = R.n_nonlinear; I.first_failed = ~0ull;
+    std::vector<uint8_t> seen(R.n_wires, 0);
+    auto mark = [&](const ConsSet &S, uint64_t base) {
+        for (uint32_t i : S.eq) seen[base + i] = 1;
+        for (const ConsTerm &t : S.kc) { seen[base + t.idx] = 1; if (cc_kind(t.coef) == CC_RCBIT || cc_payload(t.coef) != 0) seen[0] = 1; }
+        for (const ConsTerm &t : S.terms) seen[t.idx == CONS_ONE ? 0 : base + t.idx] = 1;
+    };
+    mark(R.flat, 0);
+    for (uint64_t b : R.bases) mark(R.round, b);
+    for (uint8_t v : seen) I.signals_read += v;
+    C.flat = upload_cons(C, R.flat); C.round = upload_cons(C, R.round);
+    C.konst = upload(R.konst); C.allocs.push_back(C.konst);
+    C.bases = upload(R.bases); C.allocs.push_back(C.bases); C.n_blocks = (uint32_t)R.bases.size();
+    CU(cudaMalloc(&C.rep, 24)); C.allocs.push_back(C.rep);
+    C.ready = true;
+    return C;
+}
+
+int pob_r1cs_check(pob_handle *h, uint32_t index, pob_check_report *out) {
+    if (!h || !out) return fail(POB_E_BAD_ARG, "pob_r1cs_check: null argument");
+    uint64_t *s = nullptr; int rc = resident_slot(h, index, &s); if (rc) return rc;
+    try {
+        CU(cudaSetDevice(h->device));
+        check_sets(h, ensure_r1cs(h), s, out);          // the plan has no hint records, so every record id is a row index
+    } catch (const std::exception &e) { return fail(POB_E_CUDA, std::string("pob_r1cs_check: ") + e.what()); }
+    return POB_OK;
+}
+
+int pob_r1cs_products(pob_handle *h, uint32_t index, uint64_t first_row, uint64_t n_rows, void *a, void *b, void *c, void *consumer_stream) {
+    if (!h) return fail(POB_E_BAD_ARG, "pob_r1cs_products: null handle");
+    uint64_t *s = nullptr; int rc = resident_slot(h, index, &s); if (rc) return rc;
+    try {
+        CU(cudaSetDevice(h->device));
+        pob_handle::DevCons &C = ensure_r1cs(h);
+        const uint64_t rows = C.info.n_constraints;
+        if (first_row > rows || n_rows > rows - first_row) return fail(POB_E_RANGE, "pob_r1cs_products: rows beyond the end of the system");
+        if (n_rows == 0 || !(a || b || c)) return POB_OK;
+        const cudaStream_t st = (cudaStream_t)consumer_stream;
+        R1csArgs ra{C.flat, C.round, C.konst, s, C.bases, first_row, n_rows, (uint4 *)a, (uint4 *)b, (uint4 *)c};
+        const unsigned grid = (unsigned)std::min<uint64_t>((2 * n_rows + 255) / 256, h->n_sms * 16ull);
+        k_r1cs_products<<<grid, 256, 0, st>>>(ra);
+        CU(cudaGetLastError());
+        if (!consumer_stream) CU(cudaStreamSynchronize(st));
+    } catch (const std::exception &e) { return fail(POB_E_CUDA, std::string("pob_r1cs_products: ") + e.what()); }
     return POB_OK;
 }
 

@@ -74,6 +74,15 @@ class CheckReport(ctypes.Structure):
         return {k: (float(getattr(self, k)) if k == "ms" else int(getattr(self, k))) for k, _ in self._fields_}
 
 
+class R1csDesc(ctypes.Structure):
+    _fields_ = [("n_wires", ctypes.c_uint64), ("n_pub_out", ctypes.c_uint32), ("n_pub_in", ctypes.c_uint32), ("n_prv_in", ctypes.c_uint32),
+                ("n_labels", ctypes.c_uint64), ("n_constraints", ctypes.c_uint64), ("n_nonlinear", ctypes.c_uint64), ("n_terms", ctypes.c_uint64),
+                ("file_bytes", ctypes.c_uint64)]
+
+    def as_dict(self):
+        return {k: int(getattr(self, k)) for k, _ in self._fields_}
+
+
 _LIB = None
 
 
@@ -132,6 +141,12 @@ def lib():
         L.pob_finish.argtypes = [vp, vp, vp, vp]
         L.pob_export_batch.restype = ci
         L.pob_export_batch.argtypes = [vp, vp, u32, u32, vp, vp, vp, ctypes.POINTER(ExportStats)]
+        L.pob_write_r1cs.restype = ci
+        L.pob_write_r1cs.argtypes = [ctypes.c_char_p, vp, ci, ci, ctypes.c_char_p, ctypes.POINTER(R1csDesc)]
+        L.pob_r1cs_check.restype = ci
+        L.pob_r1cs_check.argtypes = [vp, u32, ctypes.POINTER(CheckReport)]
+        L.pob_r1cs_products.restype = ci
+        L.pob_r1cs_products.argtypes = [vp, u32, u64, u64, vp, vp, vp, vp]
         L.pob_pow_grind.restype = ci
         L.pob_pow_grind.argtypes = [ci, vp, vp, vp, u32, u64, vp, ctypes.POINTER(u64)]
         L.pob_last_error.restype = ctypes.c_char_p
@@ -272,6 +287,17 @@ def write_components(main_expr, path, hcreate=False):
     return int(n.value)
 
 
+def write_r1cs(main_expr, path=None, hcreate=False, opt=0):
+    """the circuit's iden3 `.r1cs` (pob_b200.h: pob_write_r1cs), over the --O0 witness or, with opt=1, the reduced one; its wire
+    order is the order of the witness this library writes.  path=None: sizes only.  Returns the header counts and file_bytes."""
+    name, params = parse_main(main_expr)
+    pl = to_limbs(params) if params else np.zeros((1, 4), dtype=np.uint64)
+    d = R1csDesc()
+    _check(lib().pob_write_r1cs(name.encode(), pl.ctypes.data, len(params), (CREATE_HCREATE if hcreate else 0) | (CREATE_O1 if opt else 0),
+                                None if path is None else os.fsencode(path), ctypes.byref(d)))
+    return d.as_dict()
+
+
 class PinnedArray:
     """numpy view over cudaMallocHost memory (so H2D copies inside run() are asynchronous DMA)."""
 
@@ -314,7 +340,7 @@ class Circuit:
 
     def __init__(self, main_expr, device=0, hcreate=False, max_slots=0, opt=0):
         """opt=1: the reduced (`--O1`-style) witness (pob_b200.h: POB_CREATE_O1); witness_map() gives the --O0 index of each entry"""
-        self.main_expr = main_expr
+        self.main_expr, self.device = main_expr, int(device)
         self.name, self.params = parse_main(main_expr)
         self.schema = input_schema(self.name, self.params)
         pl = to_limbs(self.params) if self.params else np.zeros((1, 4), dtype=np.uint64)
@@ -457,6 +483,31 @@ class Circuit:
         _check(lib().pob_selfcheck(self._h, index, ctypes.byref(r)))
         return r.as_dict()
 
+    def r1cs_check(self, index):
+        """on-GPU evaluation of every `.r1cs` row of this handle's form (--O0 or reduced) against resident witness `index`;
+        report as selfcheck(), with first_failed a row index"""
+        r = CheckReport()
+        _check(lib().pob_r1cs_check(self._h, index, ctypes.byref(r)))
+        return r.as_dict()
+
+    def r1cs_products(self, index, first=0, count=None, stream=None, vectors="abc"):
+        """A.w, B.w, C.w of `.r1cs` rows [first, first + count) of resident witness `index`, computed on the GPU: a tuple of torch
+        uint64 CUDA tensors of shape (count, 4), the little-endian limbs of canonical field elements (None for a vector not in
+        `vectors`).  stream: a torch.cuda.Stream (or a raw cudaStream_t) ordered after the witness (e.g. by acquire(stream)); the
+        tensors are allocated and the work is enqueued on it without a host wait; None returns when done."""
+        import torch
+        if count is None:
+            if getattr(self, "_r1cs_rows", None) is None:
+                self._r1cs_rows = self.r1cs_check(index)["n_constraints"]
+            count = self._r1cs_rows - first
+        dev = torch.device("cuda", self.device)
+        handle = None if stream is None else getattr(stream, "cuda_stream", stream)
+        with torch.cuda.stream(torch.cuda.ExternalStream(handle, device=dev) if handle else torch.cuda.current_stream(dev)):
+            out = [torch.empty((count, 4), dtype=torch.uint64, device=dev) if v in vectors else None for v in "abc"]
+        ptr = [None if t is None else t.data_ptr() for t in out]
+        _check(lib().pob_r1cs_products(self._h, index, first, count, ptr[0], ptr[1], ptr[2], handle))
+        return tuple(out)
+
     def witness_map(self):
         m = np.zeros(self.n_signals, dtype=np.uint32)
         _check(lib().pob_witness_map(self._h, m.ctypes.data))
@@ -503,9 +554,15 @@ def main(argv=None):
     """CLI shim with the reference calculator's argv: `python -m pob_b200 <circuit> input.json witness.wtns`
     (reference Makefile:5-6); <circuit> is main_proof_of_burn, main_spend or a `Template(params)` expression.
     Batch form: `python -m pob_b200 <circuit> --batch in1.json in2.json ... --out DIR` evaluates all inputs in one
-    pob_run_batch and writes DIR/<name>.wtns for every accepted instance."""
+    pob_run_batch and writes DIR/<name>.wtns for every accepted instance.
+    R1CS form: `python -m pob_b200 <circuit> --r1cs out.r1cs [--O1]` writes the circuit's `.r1cs` (host only, no GPU) in the wire
+    order of the --O0 witness, or of the reduced one with --O1."""
     import sys
     argv = sys.argv[1:] if argv is None else argv
+    if len(argv) in (3, 4) and argv[1] == "--r1cs" and argv[3:] in ([], ["--O1"]):
+        d = write_r1cs(CIRCUIT_ALIASES.get(argv[0], argv[0]), argv[2], opt=1 if argv[3:] else 0)
+        print("%s: %d wires, %d constraints (%d non-linear), %d bytes" % (argv[2], d["n_wires"], d["n_constraints"], d["n_nonlinear"], d["file_bytes"]))
+        return 0
     if len(argv) >= 4 and argv[1] == "--batch" and "--out" in argv:
         k = argv.index("--out")
         files, outdir = argv[2:k], argv[k + 1]
@@ -521,7 +578,8 @@ def main(argv=None):
         return rc
     if len(argv) != 3:
         print("usage: python -m pob_b200 <main_proof_of_burn|main_spend|Template(params)> input.json witness.wtns\n"
-              "       python -m pob_b200 <circuit> --batch in1.json in2.json ... --out DIR", file=sys.stderr)
+              "       python -m pob_b200 <circuit> --batch in1.json in2.json ... --out DIR\n"
+              "       python -m pob_b200 <circuit> --r1cs out.r1cs [--O1]", file=sys.stderr)
         return 2
     c = Circuit(CIRCUIT_ALIASES.get(argv[0], argv[0]), max_slots=1)
     res = c.run([json.load(open(argv[1]))])
