@@ -242,6 +242,22 @@ int pob_r1cs_check(pob_handle *h, uint32_t index, pob_check_report *out);
  * witness (pob_acquire on it, or a finished pob_run_batch).  first_row + n_rows beyond the row count: POB_E_RANGE. */
 int pob_r1cs_products(pob_handle *h, uint32_t index, uint64_t first_row, uint64_t n_rows, void *a, void *b, void *c, void *consumer_stream);
 
+/* ---- the second stage: the Groth16 quotient evaluations (the scalars of the prover's H multi-exponentiation) --------------
+ * Follows snarkjs `groth16 prove` as far as it is known; the match with snarkjs / rapidsnark is unverified (INTEGRATION.md §3(e)).
+ * Field BN254 Fr, p - 1 = 2^28 t.  w28 = 5^t (5: the smallest quadratic non-residue), w_k = w28^(2^(28-k)).
+ * m = .r1cs rows of the handle's form, n_pub = n_pub_out + n_pub_in (= n_outputs).  Domain: n = 2^log_n, the smallest power of two
+ * >= m + n_pub + 1, omega = w_log_n; log_n > 28 is POB_E_RANGE.  Row vectors of length n: rows [0, m) are A.w, B.w, C.w as
+ * pob_r1cs_products returns them; row m + s (s = 0 .. n_pub) has a = w[s], b = c = 0; every other row is 0.  A^, B^, C^ are the
+ * polynomials of degree < n with A^(omega^k) = a_k.  Coset shift g = w_(log_n + 1) (g^n = -1) when log_n < 28, g = 25 (nqr^2) when
+ * log_n = 28.  Output q[i] = A^(g omega^i) B^(g omega^i) - C^(g omega^i), i = 0 .. n - 1, natural order, canonical 32-byte LE.
+ * snarkjs derives C on the domain as A o B; both agree on a witness that satisfies the rows. */
+/* log_n of the handle's domain (builds the row plan on first use, like pob_r1cs_check) */
+int pob_r1cs_domain(pob_handle *h, uint32_t *log_n);
+/* q[0..n) of resident witness `index` into `out` (n x 32 B); `work` is caller scratch of 2 n x 32 B, not overlapping out (else
+ * POB_E_BAD_ARG, as is a null out or work).  consumer_stream: as pob_r1cs_products (NULL = return when done; else enqueued, no host
+ * wait, nothing allocated).  The first call builds the root and coset tables (at most 2 MB), freed by pob_destroy. */
+int pob_r1cs_quotient(pob_handle *h, uint32_t index, void *out, void *work, void *consumer_stream);
+
 /* ---- the step just before the path (SURVEY.md 8(f) rank 3) ------------------------------------------------------
  * replaces: find_burn_key() of the reference input generator (tests/main.py:47-56): starting at start_key, find the
  * first burnKey >= start_key whose keccak256(burnKey[32 BE] | revealAmount[32 BE] | burnExtraCommitment[32 BE] |

@@ -27,6 +27,7 @@
 #include "../../include/pob_b200.h"
 #include "compiler.h"
 #include "kernels.cuh"
+#include "ntt.cuh"
 #include "r1cs.h"
 
 using namespace pob;
@@ -228,6 +229,8 @@ struct pob_handle {
         bool ready = false; ConsView flat{}, round{}; Fr *konst = nullptr; uint64_t *bases = nullptr; uint32_t n_blocks = 0;
         unsigned long long *rep = nullptr; std::vector<void *> allocs; pob_check_report info{};
     } cons, r1cs;
+    // root and coset tables of pob_r1cs_quotient (ntt.cuh), built on first use for the domain of the .r1cs rows
+    struct DevNtt { bool ready = false; uint32_t log_n = 0; NttTables t{}; std::vector<void *> allocs; } ntt;
 };
 
 static void cons_info(const Program &P, pob_check_report *r) {
@@ -565,6 +568,7 @@ void pob_destroy(pob_handle *h) {
     delete h->exporter; h->exporter = nullptr;
     for (void *p : h->cons.allocs) cudaFree(p);
     for (void *p : h->r1cs.allocs) cudaFree(p);
+    for (void *p : h->ntt.allocs) cudaFree(p);
     if (h->s_eval) cudaStreamSynchronize(h->s_eval);
     if (h->s_exp2) cudaStreamSynchronize(h->s_exp2);
     if (h->s_exp) cudaStreamSynchronize(h->s_exp);
@@ -1084,6 +1088,98 @@ int pob_r1cs_products(pob_handle *h, uint32_t index, uint64_t first_row, uint64_
         CU(cudaGetLastError());
         if (!consumer_stream) CU(cudaStreamSynchronize(st));
     } catch (const std::exception &e) { return fail(POB_E_CUDA, std::string("pob_r1cs_products: ") + e.what()); }
+    return POB_OK;
+}
+
+// ---- the Groth16 quotient (ntt.cuh) ----------------------------------------------------------------------------------
+// log2 of the smallest power of two >= rows + public signals + 1 (snarkjs's domain); false beyond 2^28
+static bool r1cs_log_n(pob_handle *h, uint32_t *log_n) {
+    const uint64_t need = ensure_r1cs(h).info.n_constraints + h->P.n_outputs + 1;
+    uint32_t L = 0;
+    while ((1ull << L) < need) L++;
+    *log_n = L;
+    return L <= NTT_MAX_LOG;
+}
+
+static const NttTables &ensure_ntt(pob_handle *h, uint32_t L) {
+    pob_handle::DevNtt &N = h->ntt;
+    if (N.ready) return N.t;
+    auto up = [&](const std::vector<Fr> &v) { Fr *d = upload(v); N.allocs.push_back(d); return (const Fr *)d; };
+    std::vector<Fr> v;
+    const Fr one = fr_to_mont(fr_from_u64(1)), w28 = ntt_w28_host();
+    Fr w14 = w28, w11 = w28;
+    for (uint32_t k = 0; k < NTT_TW_LOG; k++) w14 = fr_mont(w14, w14);
+    for (uint32_t k = 0; k < NTT_MAX_LOG - NTT_TILE_LOG; k++) w11 = fr_mont(w11, w11);
+    ntt_powers(v, 1u << NTT_TW_LOG, w28, one); N.t.w_lo = up(v);
+    ntt_powers(v, 1u << (NTT_MAX_LOG - NTT_TW_LOG), w14, one); N.t.w_hi = up(v);
+    ntt_powers(v, 1u << (NTT_TILE_LOG - 1), w11, one); N.t.loc = up(v);
+    ntt_powers(v, 1u << (NTT_TILE_LOG - 1), fr_to_mont(fr_inv(fr_from_mont(w11))), one); N.t.loc_inv = up(v);
+    const Fr g = ntt_shift_host(L);
+    Fr gs = g;
+    N.t.g_log = (L + 1) / 2;
+    for (uint32_t k = 0; k < N.t.g_log; k++) gs = fr_mont(gs, gs);
+    ntt_powers(v, 1ull << N.t.g_log, g, one); N.t.g_lo = up(v);
+    ntt_powers(v, 1ull << (L - N.t.g_log), gs, fr_to_mont(fr_inv(fr_from_u64(1ull << L)))); N.t.g_hi = up(v);   // g^(t 2^g_log) / n
+    const int smem = 32 << NTT_TILE_LOG;
+    CU(cudaFuncSetAttribute(k_ntt_inv, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    CU(cudaFuncSetAttribute(k_ntt_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    N.log_n = L; N.ready = true;
+    return N.t;
+}
+
+int pob_r1cs_domain(pob_handle *h, uint32_t *log_n) {
+    if (!h || !log_n) return fail(POB_E_BAD_ARG, "pob_r1cs_domain: null argument");
+    try {
+        CU(cudaSetDevice(h->device));
+        if (!r1cs_log_n(h, log_n)) return fail(POB_E_RANGE, "pob_r1cs_domain: the domain exceeds 2^28 points");
+    } catch (const std::exception &e) { return fail(POB_E_CUDA, std::string("pob_r1cs_domain: ") + e.what()); }
+    return POB_OK;
+}
+
+int pob_r1cs_quotient(pob_handle *h, uint32_t index, void *out, void *work, void *consumer_stream) {
+    if (!h || !out || !work) return fail(POB_E_BAD_ARG, "pob_r1cs_quotient: null argument");
+    uint64_t *s = nullptr; int rc = resident_slot(h, index, &s); if (rc) return rc;
+    try {
+        CU(cudaSetDevice(h->device));
+        pob_handle::DevCons &C = ensure_r1cs(h);
+        uint32_t L = 0;
+        if (!r1cs_log_n(h, &L)) return fail(POB_E_RANGE, "pob_r1cs_quotient: the domain exceeds 2^28 points");
+        const NttTables &T = ensure_ntt(h, L);
+        const uint64_t n = 1ull << L, m = C.info.n_constraints, np1 = h->P.n_outputs + 1;
+        const uintptr_t o = (uintptr_t)out, w = (uintptr_t)work;
+        if (o < w + 64 * n && w < o + 32 * n) return fail(POB_E_BAD_ARG, "pob_r1cs_quotient: work overlaps out");
+        const cudaStream_t st = (cudaStream_t)consumer_stream;
+        uint4 *va = (uint4 *)out, *vb = (uint4 *)work, *vc = vb + 2 * n;        // 2 uint4 per entry
+        // rows: [0, m) the products, m + s (s <= n_pub) a = w[s], the rest 0
+        if (m) {
+            R1csArgs ra{C.flat, C.round, C.konst, s, C.bases, 0, m, va, vb, vc};
+            k_r1cs_products<<<(unsigned)std::min<uint64_t>((2 * m + 255) / 256, h->n_sms * 16ull), 256, 0, st>>>(ra);
+            CU(cudaGetLastError());
+        }
+        CU(cudaMemcpyAsync(va + 2 * m, s, np1 * 32, cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemsetAsync(va + 2 * (m + np1), 0, (n - m - np1) * 32, st));
+        CU(cudaMemsetAsync(vb + 2 * m, 0, (n - m) * 32, st));
+        CU(cudaMemsetAsync(vc + 2 * m, 0, (n - m) * 32, st));
+        const uint32_t tl = std::min(L, NTT_TILE_LOG);
+        const std::vector<uint32_t> k = ntt_plan(L, tl);
+        const uint32_t P = (uint32_t)k.size(), grid = (uint32_t)(n >> tl), smem = 32u << tl;
+        for (uint4 *x : {va, vb, vc}) {
+            uint32_t blk = L;
+            for (uint32_t i = 0; i < P; i++) {                                   // inverse, then g^k / n: coefficients on the coset
+                const NttPass p{x, L, blk, k[i], tl, i + 1 == P, nullptr, nullptr, nullptr, T};
+                k_ntt_inv<<<grid, NTT_THREADS, smem, st>>>(p);
+                blk -= k[i];
+            }
+            for (uint32_t i = P; i-- > 0;) {                                     // forward: the values on the coset
+                blk += k[i];
+                NttPass p{x, L, blk, k[i], tl, 0, nullptr, nullptr, nullptr, T};
+                if (x == vc && i == 0) { p.last = 1; p.a = va; p.b = vb; p.q = va; }   // q = A.B - C, over A in out
+                k_ntt_fwd<<<grid, NTT_THREADS, smem, st>>>(p);
+            }
+        }
+        CU(cudaGetLastError());
+        if (!consumer_stream) CU(cudaStreamSynchronize(st));
+    } catch (const std::exception &e) { return fail(POB_E_CUDA, std::string("pob_r1cs_quotient: ") + e.what()); }
     return POB_OK;
 }
 

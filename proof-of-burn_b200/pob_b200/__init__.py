@@ -147,6 +147,10 @@ def lib():
         L.pob_r1cs_check.argtypes = [vp, u32, ctypes.POINTER(CheckReport)]
         L.pob_r1cs_products.restype = ci
         L.pob_r1cs_products.argtypes = [vp, u32, u64, u64, vp, vp, vp, vp]
+        L.pob_r1cs_domain.restype = ci
+        L.pob_r1cs_domain.argtypes = [vp, ctypes.POINTER(u32)]
+        L.pob_r1cs_quotient.restype = ci
+        L.pob_r1cs_quotient.argtypes = [vp, u32, vp, vp, vp]
         L.pob_pow_grind.restype = ci
         L.pob_pow_grind.argtypes = [ci, vp, vp, vp, u32, u64, vp, ctypes.POINTER(u64)]
         L.pob_last_error.restype = ctypes.c_char_p
@@ -507,6 +511,31 @@ class Circuit:
         ptr = [None if t is None else t.data_ptr() for t in out]
         _check(lib().pob_r1cs_products(self._h, index, first, count, ptr[0], ptr[1], ptr[2], handle))
         return tuple(out)
+
+    def r1cs_domain(self):
+        """log2 of the quotient's domain size n: the smallest power of two >= rows + public signals + 1 (pob_r1cs_domain)"""
+        v = ctypes.c_uint32(0)
+        _check(lib().pob_r1cs_domain(self._h, ctypes.byref(v)))
+        return int(v.value)
+
+    def r1cs_quotient(self, index, stream=None, out=None, work=None):
+        """the Groth16 quotient evaluations of resident witness `index` on the GPU (pob_b200.h: pob_r1cs_quotient): a torch uint64
+        CUDA tensor of shape (n, 4), q[i] = A^(g w^i) B^(g w^i) - C^(g w^i) as the limbs of canonical field elements.  out (n x 32 B)
+        and work (2 n x 32 B of scratch) are allocated on `stream` unless given; stream as in r1cs_products."""
+        import torch
+        n = 1 << self.r1cs_domain()
+        dev = torch.device("cuda", self.device)
+        handle = None if stream is None else getattr(stream, "cuda_stream", stream)
+        with torch.cuda.stream(torch.cuda.ExternalStream(handle, device=dev) if handle else torch.cuda.current_stream(dev)):
+            if out is None:
+                out = torch.empty((n, 4), dtype=torch.uint64, device=dev)
+            if work is None:
+                work = torch.empty((2 * n, 4), dtype=torch.uint64, device=dev)
+        for t, need, what in ((out, 32 * n, "out"), (work, 64 * n, "work")):
+            if not t.is_cuda or not t.is_contiguous() or t.numel() * t.element_size() < need:
+                raise ValueError("r1cs_quotient: %s must be a contiguous CUDA tensor of at least %d bytes" % (what, need))
+        _check(lib().pob_r1cs_quotient(self._h, index, out.data_ptr(), work.data_ptr(), handle))
+        return out
 
     def witness_map(self):
         m = np.zeros(self.n_signals, dtype=np.uint32)
