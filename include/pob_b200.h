@@ -237,7 +237,9 @@ int pob_write_r1cs(const char *main_name, const uint64_t *params, int nparams, i
  * n_hints / n_hint_failed are 0, signals_read = wires referenced.  The first call builds and uploads the row plan. */
 int pob_r1cs_check(pob_handle *h, uint32_t index, pob_check_report *out);
 /* the first stage of a GPU Groth16 prover: rows [first_row, first_row + n_rows) of the .r1cs, a[k], b[k], c[k] = A.w, B.w, C.w of
- * row first_row + k as 32-byte canonical LE field elements, into caller device buffers (any may be NULL: not computed).
+ * row first_row + k as 32-byte canonical LE field elements (a row's constants multiply w[0], as in the file, so these are the rows'
+ * linear forms on any witness), into caller device buffers (any may be NULL: not computed), each
+ * 16-byte aligned (else POB_E_BAD_ARG, before anything is enqueued).
  * consumer_stream NULL: returns when done; else (a cudaStream_t) enqueued on that stream, which the caller has ordered after the
  * witness (pob_acquire on it, or a finished pob_run_batch).  first_row + n_rows beyond the row count: POB_E_RANGE. */
 int pob_r1cs_products(pob_handle *h, uint32_t index, uint64_t first_row, uint64_t n_rows, void *a, void *b, void *c, void *consumer_stream);
@@ -254,7 +256,7 @@ int pob_r1cs_products(pob_handle *h, uint32_t index, uint64_t first_row, uint64_
 /* log_n of the handle's domain (builds the row plan on first use, like pob_r1cs_check) */
 int pob_r1cs_domain(pob_handle *h, uint32_t *log_n);
 /* q[0..n) of resident witness `index` into `out` (n x 32 B); `work` is caller scratch of 2 n x 32 B, not overlapping out (else
- * POB_E_BAD_ARG, as is a null out or work).  consumer_stream: as pob_r1cs_products (NULL = return when done; else enqueued, no host
+ * POB_E_BAD_ARG, as is a null out or work, or one that is not 16-byte aligned).  consumer_stream: as pob_r1cs_products (NULL = return when done; else enqueued, no host
  * wait, nothing allocated).  The first call builds the root and coset tables (at most 2 MB), freed by pob_destroy. */
 int pob_r1cs_quotient(pob_handle *h, uint32_t index, void *out, void *work, void *consumer_stream);
 

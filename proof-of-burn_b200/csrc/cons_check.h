@@ -19,8 +19,10 @@ struct ConsView {                                    // one ConsSet in device (o
     POB_HD uint64_t n_records() const { return n_eq + n_kc + n_r1; }
 };
 
-POB_HD Fr cons_load(const uint64_t *wit, uint64_t base, uint32_t idx) {
-    if (idx == CONS_ONE) return fr_from_u64(1);
+// CONS_ONE is the constant wire w[0]: `one` is its value, 1 on every witness the circuit accepts (the .r1cs products pass the
+// witness's own w[0], so that they stay the rows' linear forms on any witness)
+POB_HD Fr cons_load(const uint64_t *wit, uint64_t base, uint32_t idx, const Fr &one = fr_from_u64(1)) {
+    if (idx == CONS_ONE) return one;
     return vm_load_val(wit + 4ull * (base + idx));
 }
 POB_HD bool cons_eq_ok(const uint64_t *wit, uint64_t base, uint32_t a, uint32_t b) {
@@ -38,10 +40,10 @@ POB_HD Fr cons_coef_value(uint32_t c, const Fr *konst, uint64_t rc) {
 POB_HD bool cons_kc_ok(const uint64_t *wit, uint64_t base, const ConsTerm t, const Fr *konst, uint64_t rc) {
     return fr_eq(cons_load(wit, base, t.idx), cons_coef_value(t.coef, konst, rc));
 }
-POB_HD Fr cons_lc(const uint64_t *wit, uint64_t base, const ConsTerm *t, uint32_t n, const Fr *konst) {
+POB_HD Fr cons_lc(const uint64_t *wit, uint64_t base, const ConsTerm *t, uint32_t n, const Fr *konst, const Fr &one = fr_from_u64(1)) {
     Fr acc = fr_zero();
     for (uint32_t i = 0; i < n; i++) {
-        const Fr v = cons_load(wit, base, t[i].idx);
+        const Fr v = cons_load(wit, base, t[i].idx, one);
         const uint32_t k = cc_kind(t[i].coef), p = cc_payload(t[i].coef);
         if (k == CC_POS) acc = fr_add(acc, p == 1 ? v : fr_mul(v, fr_from_u64(p)));
         else if (k == CC_NEG) acc = fr_sub(acc, p == 1 ? v : fr_mul(v, fr_from_u64(p)));

@@ -607,6 +607,7 @@ __global__ void __launch_bounds__(256) k_r1cs_products(const R1csArgs a) {
     const uint32_t h = threadIdx.x & 1u;
     const uint64_t nf = a.flat.n_records(), per = a.round.n_records();
     const bool want_ab = a.a || a.b;
+    const Fr w0 = cons_load(a.wit, 0, 0);                                   // constants are multiples of w[0], as in the file
     for (uint64_t k = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 1; k < a.n; k += ((uint64_t)gridDim.x * blockDim.x) >> 1) {
         uint64_t r = a.first + k, base = 0, rc = 0;
         const bool in_round = r >= nf;
@@ -614,15 +615,15 @@ __global__ void __launch_bounds__(256) k_r1cs_products(const R1csArgs a) {
         const ConsView V = in_round ? a.round : a.flat;
         Fr A = fr_zero(), B = fr_zero(), C;
         if (r < V.n_eq) {                                                   // C = w[a] - w[b]
-            C = fr_sub(cons_load(a.wit, base, V.eq[2 * r]), cons_load(a.wit, base, V.eq[2 * r + 1]));
+            C = fr_sub(cons_load(a.wit, base, V.eq[2 * r], w0), cons_load(a.wit, base, V.eq[2 * r + 1], w0));
         } else if (r < V.n_eq + V.n_kc) {                                   // C = w[a] - k w0
             const ConsTerm t = V.kc[r - V.n_eq];
-            C = fr_sub(cons_load(a.wit, base, t.idx), cons_coef_value(t.coef, a.konst, rc));
+            C = fr_sub(cons_load(a.wit, base, t.idx, w0), fr_mul(cons_coef_value(t.coef, a.konst, rc), w0));
         } else {
             const ConsR1 rec = V.r1[r - V.n_eq - V.n_kc];
             const ConsTerm *t = V.terms + rec.off;
-            C = a.c ? cons_lc(a.wit, base, t + rec.na + rec.nb, r1_nc(rec), a.konst) : fr_zero();
-            if (want_ab && rec.na) { A = cons_lc(a.wit, base, t, rec.na, a.konst); B = cons_lc(a.wit, base, t + rec.na, rec.nb, a.konst); }
+            C = a.c ? cons_lc(a.wit, base, t + rec.na + rec.nb, r1_nc(rec), a.konst, w0) : fr_zero();
+            if (want_ab && rec.na) { A = cons_lc(a.wit, base, t, rec.na, a.konst, w0); B = cons_lc(a.wit, base, t + rec.na, rec.nb, a.konst, w0); }
         }
         if (a.a) st_half(a.a, k, h, A);
         if (a.b) st_half(a.b, k, h, B);

@@ -164,13 +164,16 @@ __global__ void __launch_bounds__(NTT_THREADS) k_ntt_fwd(const NttPass p) {
 // ---- host side ---------------------------------------------------------------------------------------------------------------
 // stages per pass of a 2^L transform with 2^T-entry tiles, in the order of the inverse transform (the forward one runs them in
 // reverse): as few passes as keep every pass but the contiguous last one at <= T - 2 stages (runs of >= 4 entries = 128 bytes),
-// balanced, the largest last
+// balanced, the largest last.  A balanced pass above T - 2 (only 10 + 10 at L = 20 for T = 11) gives its excess to the last pass,
+// which still has at most T stages because the pass count allows it.
 static std::vector<uint32_t> ntt_plan(uint32_t L, uint32_t T) {
     uint32_t q = 0;
     while (L > T + q * (T - 2)) q++;
     const uint32_t P = q + 1;
     std::vector<uint32_t> k(P, L / P);
     for (uint32_t i = 0; i < L % P; i++) k[P - 1 - i]++;
+    for (uint32_t i = 0; i + 1 < P; i++)
+        if (k[i] > T - 2) { k[P - 1] += k[i] - (T - 2); k[i] = T - 2; }
     return k;
 }
 
@@ -196,6 +199,68 @@ static Fr ntt_shift_host(uint32_t L) {
     Fr g = ntt_w28_host();
     for (uint32_t k = L + 1; k < NTT_MAX_LOG; k++) g = fr_mont(g, g);
     return g;
+}
+
+// the tables of NttTables for a 2^L domain, on the host, Montgomery form
+struct NttHostTables {
+    std::vector<Fr> w_lo, w_hi, loc, loc_inv, g_lo, g_hi;
+    uint32_t g_log;
+};
+static NttHostTables ntt_host_tables(uint32_t L) {
+    NttHostTables H;
+    const Fr one = fr_to_mont(fr_from_u64(1)), w28 = ntt_w28_host();
+    Fr w14 = w28, w11 = w28;
+    for (uint32_t k = 0; k < NTT_TW_LOG; k++) w14 = fr_mont(w14, w14);
+    for (uint32_t k = 0; k < NTT_MAX_LOG - NTT_TILE_LOG; k++) w11 = fr_mont(w11, w11);
+    ntt_powers(H.w_lo, 1u << NTT_TW_LOG, w28, one);
+    ntt_powers(H.w_hi, 1u << (NTT_MAX_LOG - NTT_TW_LOG), w14, one);
+    ntt_powers(H.loc, 1u << (NTT_TILE_LOG - 1), w11, one);
+    ntt_powers(H.loc_inv, 1u << (NTT_TILE_LOG - 1), fr_to_mont(fr_inv(fr_from_mont(w11))), one);
+    const Fr g = ntt_shift_host(L);
+    Fr gs = g;
+    H.g_log = (L + 1) / 2;
+    for (uint32_t k = 0; k < H.g_log; k++) gs = fr_mont(gs, gs);
+    ntt_powers(H.g_lo, 1ull << H.g_log, g, one);
+    ntt_powers(H.g_hi, 1ull << (L - H.g_log), gs, fr_to_mont(fr_inv(fr_from_u64(1ull << L))));   // g^(t 2^g_log) / n
+    return H;
+}
+
+// once per process and device, before the first launch: both kernels use 32 << NTT_TILE_LOG bytes of dynamic shared memory
+static cudaError_t ntt_init_kernels() {
+    const int smem = 32 << NTT_TILE_LOG;
+    cudaError_t e = cudaFuncSetAttribute(k_ntt_inv, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_ntt_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    return e;
+}
+
+// enqueue the inverse transform of the 2^L entries at x (2 uint4 each) with 2^T-entry tiles, natural order in, bit-reversed
+// order out; its last pass multiplies coefficient k by g^k / n
+static cudaError_t ntt_inverse_coset(uint4 *x, uint32_t L, uint32_t T, const NttTables &t, cudaStream_t st) {
+    const std::vector<uint32_t> k = ntt_plan(L, T);
+    const uint32_t P = (uint32_t)k.size(), grid = (uint32_t)((1ull << L) >> T), smem = 32u << T;
+    uint32_t blk = L;
+    for (uint32_t i = 0; i < P; i++) {
+        const NttPass p{x, L, blk, k[i], T, i + 1 == P, nullptr, nullptr, nullptr, t};
+        k_ntt_inv<<<grid, NTT_THREADS, smem, st>>>(p);
+        blk -= k[i];
+    }
+    return cudaGetLastError();
+}
+
+// enqueue the forward transform of x, bit-reversed order in, natural order out; with q set, its last pass writes q = A.B - x's
+// values instead of them (A, B canonical, natural order; q may be a)
+static cudaError_t ntt_forward(uint4 *x, uint32_t L, uint32_t T, const NttTables &t, cudaStream_t st,
+                               const uint4 *a = nullptr, const uint4 *b = nullptr, uint4 *q = nullptr) {
+    const std::vector<uint32_t> k = ntt_plan(L, T);
+    const uint32_t P = (uint32_t)k.size(), grid = (uint32_t)((1ull << L) >> T), smem = 32u << T;
+    uint32_t blk = 0;
+    for (uint32_t i = P; i-- > 0;) {
+        blk += k[i];
+        NttPass p{x, L, blk, k[i], T, 0, nullptr, nullptr, nullptr, t};
+        if (q && i == 0) { p.last = 1; p.a = a; p.b = b; p.q = q; }
+        k_ntt_fwd<<<grid, NTT_THREADS, smem, st>>>(p);
+    }
+    return cudaGetLastError();
 }
 
 }  // namespace

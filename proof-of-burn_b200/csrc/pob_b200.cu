@@ -1072,8 +1072,15 @@ int pob_r1cs_check(pob_handle *h, uint32_t index, pob_check_report *out) {
     return POB_OK;
 }
 
+// the row and transform kernels access caller buffers as uint4
+static bool misaligned16(std::initializer_list<const void *> bufs) {
+    for (const void *p : bufs) if ((uintptr_t)p & 15) return true;
+    return false;
+}
+
 int pob_r1cs_products(pob_handle *h, uint32_t index, uint64_t first_row, uint64_t n_rows, void *a, void *b, void *c, void *consumer_stream) {
     if (!h) return fail(POB_E_BAD_ARG, "pob_r1cs_products: null handle");
+    if (misaligned16({a, b, c})) return fail(POB_E_BAD_ARG, "pob_r1cs_products: a, b and c must be 16-byte aligned");
     uint64_t *s = nullptr; int rc = resident_slot(h, index, &s); if (rc) return rc;
     try {
         CU(cudaSetDevice(h->device));
@@ -1105,24 +1112,10 @@ static const NttTables &ensure_ntt(pob_handle *h, uint32_t L) {
     pob_handle::DevNtt &N = h->ntt;
     if (N.ready) return N.t;
     auto up = [&](const std::vector<Fr> &v) { Fr *d = upload(v); N.allocs.push_back(d); return (const Fr *)d; };
-    std::vector<Fr> v;
-    const Fr one = fr_to_mont(fr_from_u64(1)), w28 = ntt_w28_host();
-    Fr w14 = w28, w11 = w28;
-    for (uint32_t k = 0; k < NTT_TW_LOG; k++) w14 = fr_mont(w14, w14);
-    for (uint32_t k = 0; k < NTT_MAX_LOG - NTT_TILE_LOG; k++) w11 = fr_mont(w11, w11);
-    ntt_powers(v, 1u << NTT_TW_LOG, w28, one); N.t.w_lo = up(v);
-    ntt_powers(v, 1u << (NTT_MAX_LOG - NTT_TW_LOG), w14, one); N.t.w_hi = up(v);
-    ntt_powers(v, 1u << (NTT_TILE_LOG - 1), w11, one); N.t.loc = up(v);
-    ntt_powers(v, 1u << (NTT_TILE_LOG - 1), fr_to_mont(fr_inv(fr_from_mont(w11))), one); N.t.loc_inv = up(v);
-    const Fr g = ntt_shift_host(L);
-    Fr gs = g;
-    N.t.g_log = (L + 1) / 2;
-    for (uint32_t k = 0; k < N.t.g_log; k++) gs = fr_mont(gs, gs);
-    ntt_powers(v, 1ull << N.t.g_log, g, one); N.t.g_lo = up(v);
-    ntt_powers(v, 1ull << (L - N.t.g_log), gs, fr_to_mont(fr_inv(fr_from_u64(1ull << L)))); N.t.g_hi = up(v);   // g^(t 2^g_log) / n
-    const int smem = 32 << NTT_TILE_LOG;
-    CU(cudaFuncSetAttribute(k_ntt_inv, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    CU(cudaFuncSetAttribute(k_ntt_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    const NttHostTables H = ntt_host_tables(L);
+    N.t.w_lo = up(H.w_lo); N.t.w_hi = up(H.w_hi); N.t.loc = up(H.loc); N.t.loc_inv = up(H.loc_inv);
+    N.t.g_lo = up(H.g_lo); N.t.g_hi = up(H.g_hi); N.t.g_log = H.g_log;
+    CU(ntt_init_kernels());
     N.log_n = L; N.ready = true;
     return N.t;
 }
@@ -1138,6 +1131,7 @@ int pob_r1cs_domain(pob_handle *h, uint32_t *log_n) {
 
 int pob_r1cs_quotient(pob_handle *h, uint32_t index, void *out, void *work, void *consumer_stream) {
     if (!h || !out || !work) return fail(POB_E_BAD_ARG, "pob_r1cs_quotient: null argument");
+    if (misaligned16({out, work})) return fail(POB_E_BAD_ARG, "pob_r1cs_quotient: out and work must be 16-byte aligned");
     uint64_t *s = nullptr; int rc = resident_slot(h, index, &s); if (rc) return rc;
     try {
         CU(cudaSetDevice(h->device));
@@ -1161,23 +1155,11 @@ int pob_r1cs_quotient(pob_handle *h, uint32_t index, void *out, void *work, void
         CU(cudaMemsetAsync(vb + 2 * m, 0, (n - m) * 32, st));
         CU(cudaMemsetAsync(vc + 2 * m, 0, (n - m) * 32, st));
         const uint32_t tl = std::min(L, NTT_TILE_LOG);
-        const std::vector<uint32_t> k = ntt_plan(L, tl);
-        const uint32_t P = (uint32_t)k.size(), grid = (uint32_t)(n >> tl), smem = 32u << tl;
-        for (uint4 *x : {va, vb, vc}) {
-            uint32_t blk = L;
-            for (uint32_t i = 0; i < P; i++) {                                   // inverse, then g^k / n: coefficients on the coset
-                const NttPass p{x, L, blk, k[i], tl, i + 1 == P, nullptr, nullptr, nullptr, T};
-                k_ntt_inv<<<grid, NTT_THREADS, smem, st>>>(p);
-                blk -= k[i];
-            }
-            for (uint32_t i = P; i-- > 0;) {                                     // forward: the values on the coset
-                blk += k[i];
-                NttPass p{x, L, blk, k[i], tl, 0, nullptr, nullptr, nullptr, T};
-                if (x == vc && i == 0) { p.last = 1; p.a = va; p.b = vb; p.q = va; }   // q = A.B - C, over A in out
-                k_ntt_fwd<<<grid, NTT_THREADS, smem, st>>>(p);
-            }
+        for (uint4 *x : {va, vb, vc}) {                                          // coefficients on the coset, then their values there
+            CU(ntt_inverse_coset(x, L, tl, T, st));
+            if (x == vc) CU(ntt_forward(x, L, tl, T, st, va, vb, va));           // q = A.B - C, over A in out
+            else CU(ntt_forward(x, L, tl, T, st));
         }
-        CU(cudaGetLastError());
         if (!consumer_stream) CU(cudaStreamSynchronize(st));
     } catch (const std::exception &e) { return fail(POB_E_CUDA, std::string("pob_r1cs_quotient: ") + e.what()); }
     return POB_OK;

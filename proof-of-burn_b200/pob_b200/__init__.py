@@ -532,8 +532,8 @@ class Circuit:
             if work is None:
                 work = torch.empty((2 * n, 4), dtype=torch.uint64, device=dev)
         for t, need, what in ((out, 32 * n, "out"), (work, 64 * n, "work")):
-            if not t.is_cuda or not t.is_contiguous() or t.numel() * t.element_size() < need:
-                raise ValueError("r1cs_quotient: %s must be a contiguous CUDA tensor of at least %d bytes" % (what, need))
+            if not t.is_cuda or t.device != dev or not t.is_contiguous() or t.numel() * t.element_size() < need:
+                raise ValueError("r1cs_quotient: %s must be a contiguous tensor on %s of at least %d bytes" % (what, dev, need))
         _check(lib().pob_r1cs_quotient(self._h, index, out.data_ptr(), work.data_ptr(), handle))
         return out
 
