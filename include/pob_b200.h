@@ -138,8 +138,15 @@ int pob_run_batch_retain(pob_handle *h, const uint64_t *inputs, uint32_t n, uint
  *                consumer_stream == NULL: returns when the witness is complete in HBM (host wait);
  *                else (a cudaStream_t): returns at once and makes that stream wait for the witness on the GPU.
  *   pob_release  the consumer is done with instance `index`; consumer_stream (or NULL = already finished on the
- *                host) orders the reuse of the slot after the consumer's queued work.
+ *                host) orders the reuse of the slot after the consumer's queued work -- also when the reuse comes
+ *                from a later pob_submit / pob_run_batch / pob_export_batch on this handle.
  *   pob_finish   drain the batch (instances never acquired are generated and dropped), return status/outputs/digests.
+ *                A witness still held counts as released on the stream it was acquired on: its slot is reused only
+ *                after that stream's queued work, so that stream must stay valid until pob_finish returns (a witness
+ *                acquired with NULL is taken as read already).
+ * The host accessors below (pob_copy_witness, pob_write_wtns, pob_witness_device_ptr, the self-checks, and the row
+ * products / quotient with a NULL stream) wait on the host for a held witness that was acquired on a stream and is
+ * still being generated; given a stream, pob_r1cs_products / pob_r1cs_quotient make that stream wait for it instead.
  * One batch at a time per handle; the last n_slots non-released instances stay resident after pob_finish. */
 int pob_submit(pob_handle *h, const uint64_t *inputs, uint32_t n, uint32_t flags);
 int pob_acquire(pob_handle *h, uint32_t *index, void **dptr, void *consumer_stream);

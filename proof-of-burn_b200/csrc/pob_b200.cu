@@ -217,6 +217,7 @@ struct pob_handle {
         const uint64_t *inputs = nullptr; uint32_t n = 0, nchunks = 0, next_eval = 0, next_group = 0, acq_pos = 0;
         std::vector<uint32_t> plan, slot;         // instances to materialise (ascending) and their slots
         std::vector<uint8_t> st;                  // per plan entry: 0 = not handed out yet, 1 = held by the consumer, 2 = released / dropped
+        std::vector<cudaStream_t> acq_stream;     // per plan entry: the stream it was acquired on (nullptr = on the host)
         std::vector<uint32_t> group_of;           // per plan entry
         std::vector<Group> groups; std::vector<uint32_t> chunk_gend;   // groups sorted by chunk; chunk_gend[c] = one past the last group of chunks <= c
         std::vector<cudaEvent_t> e0, e1, est;     // per chunk: eval begin / end, status+outputs on the host
@@ -445,7 +446,7 @@ static int begin_batch(pob_handle *h, const uint64_t *inputs, uint32_t n, uint32
         else { B.plan.resize(n); for (uint32_t i = 0; i < n; i++) B.plan[i] = i; }
     }
     const uint32_t np = (uint32_t)B.plan.size();
-    B.slot.resize(np); B.st.assign(np, 0); B.group_of.resize(np);
+    B.slot.resize(np); B.st.assign(np, 0); B.acq_stream.assign(np, nullptr); B.group_of.resize(np);
     for (uint32_t k = 0; k < np; k++) { B.slot[k] = k % ns; h->h_witptr[k] = h->slots[B.slot[k]]; h->h_planinst[k] = B.plan[k]; }
     h->ev_used = 0;
     B.chunk_gend.assign(B.nchunks, 0);
@@ -460,9 +461,11 @@ static int begin_batch(pob_handle *h, const uint64_t *inputs, uint32_t n, uint32
     for (uint32_t c = 1; c < B.nchunks; c++) B.chunk_gend[c] = std::max(B.chunk_gend[c], B.chunk_gend[c - 1]);
     B.e0.resize(B.nchunks); B.e1.resize(B.nchunks); B.est.resize(B.nchunks);
     for (uint32_t c = 0; c < B.nchunks; c++) { B.e0[c] = pool_event(h); B.e1[c] = pool_event(h); B.est[c] = pool_event(h); }
-    // the previous batch's residency ends here: its slots are about to be reused
+    // the previous batch's residency ends here: its slots are about to be reused, but not before the consumer work its
+    // stream-ordered releases stand for (s_exp2 forks from s_exp, so it follows)
     std::fill(h->slot_owner.begin(), h->slot_owner.end(), (int64_t)-1);
-    std::fill(h->slot_rel_pending.begin(), h->slot_rel_pending.end(), (uint8_t)0);
+    for (size_t s = 0; s < h->slots.size(); s++)
+        if (h->slot_rel_pending[s]) { CU(cudaStreamWaitEvent(h->s_exp, h->slot_rel_ev[s], 0)); h->slot_rel_pending[s] = 0; }
     h->last_n = 0; h->last_status.clear();
     CU(cudaEventRecord(h->ev_start, h->s_eval));
     if (np) {
@@ -480,6 +483,10 @@ static int begin_batch(pob_handle *h, const uint64_t *inputs, uint32_t n, uint32
 static int finish_batch(pob_handle *h, uint32_t *status, uint64_t *outputs, uint64_t *digests) {
     pob_handle::Batch &B = h->B; const Program &P = h->P;
     const uint32_t n = B.n; const size_t no = std::max<uint32_t>(1, P.n_outputs);
+    // a witness still held on a consumer stream counts as released on that stream: its slot is reused (by this batch or the
+    // next) only after the consumer's queued reads
+    for (size_t k = 0; k < B.st.size(); k++)
+        if (B.st[k] == 1 && B.acq_stream[k]) { CU(cudaEventRecord(h->slot_rel_ev[B.slot[k]], B.acq_stream[k])); h->slot_rel_pending[B.slot[k]] = 1; }
     for (auto &s : B.st) s = 2;                            // whatever the consumer did not take is generated and dropped
     advance(h);
     if (B.next_eval != B.nchunks || B.next_group != B.groups.size()) throw std::runtime_error("internal: batch did not drain");
@@ -808,7 +815,7 @@ int pob_acquire(pob_handle *h, uint32_t *index, void **dptr, void *consumer_stre
         if (h->h_status[i] != 0) { *dptr = nullptr; B.st[k] = 2; B.acq_pos++; advance(h); return fail(POB_E_REJECTED, "pob_acquire: the instance failed a constraint and has no witness"); }
         if (consumer_stream) CU(cudaStreamWaitEvent((cudaStream_t)consumer_stream, B.groups[g].t1, 0));
         else CU(cudaEventSynchronize(B.groups[g].t1));
-        *dptr = h->slots[B.slot[k]]; B.st[k] = 1; B.acq_pos++;
+        *dptr = h->slots[B.slot[k]]; B.st[k] = 1; B.acq_stream[k] = (cudaStream_t)consumer_stream; B.acq_pos++;
         return POB_OK;
     } catch (const std::exception &e) { abort_batch(h); return fail(POB_E_CUDA, std::string("pob_acquire: ") + e.what()); }
 }
@@ -915,17 +922,28 @@ int pob_last_timing(const pob_handle *h, pob_timing *out) {
     *out = h->timing; return POB_OK;
 }
 
-// slot of a resident, ACCEPTED instance of the last finished batch (or of one the consumer currently holds)
-static int resident_slot(pob_handle *h, uint32_t index, uint64_t **slot) {
+// slot of a resident, ACCEPTED instance of the last finished batch (or of one the consumer currently holds).  A held witness
+// may have been acquired on a stream and still be in the making: `stream` (nullptr = the caller reads on the host or the legacy
+// stream) is made to wait for it on the GPU, else the host waits
+static int resident_slot(pob_handle *h, uint32_t index, uint64_t **slot, cudaStream_t stream = nullptr) {
     const uint32_t *st = nullptr; uint32_t n = 0;
     if (h->B.active) { st = h->h_status; n = h->B.n; } else { st = h->last_status.data(); n = h->last_n; }
     if (index >= n) return fail(POB_E_RANGE, "witness index not in the last batch");
+    const pob_handle::Group *G = nullptr;
     if (h->B.active) {
         auto it = std::lower_bound(h->B.plan.begin(), h->B.plan.end(), index);
-        if (it == h->B.plan.end() || *it != index || h->B.st[(size_t)(it - h->B.plan.begin())] != 1) return fail(POB_E_RANGE, "a batch is in flight and the consumer does not hold this witness");
+        const size_t k = (size_t)(it - h->B.plan.begin());
+        if (it == h->B.plan.end() || *it != index || h->B.st[k] != 1) return fail(POB_E_RANGE, "a batch is in flight and the consumer does not hold this witness");
+        G = &h->B.groups[h->B.group_of[k]];
     }
     if (st[index] != 0) return fail(POB_E_REJECTED, "the instance failed a circuit constraint: it has no witness");
-    for (size_t s = 0; s < h->slots.size(); s++) if (h->slot_owner[s] == (int64_t)index) { *slot = h->slots[s]; return POB_OK; }
+    for (size_t s = 0; s < h->slots.size(); s++) if (h->slot_owner[s] == (int64_t)index) {
+        if (G) {
+            const cudaError_t e = stream ? cudaStreamWaitEvent(stream, G->t1, 0) : cudaEventSynchronize(G->t1);
+            if (e != cudaSuccess) return fail(POB_E_CUDA, std::string("waiting for the witness: ") + cudaGetErrorString(e));
+        }
+        *slot = h->slots[s]; return POB_OK;
+    }
     return fail(POB_E_RANGE, "witness not resident: not materialised, released, or its slot was reused by a later instance");
 }
 
@@ -1058,6 +1076,8 @@ static pob_handle::DevCons &ensure_r1cs(pob_handle *h) {
     C.konst = upload(R.konst); C.allocs.push_back(C.konst);
     C.bases = upload(R.bases); C.allocs.push_back(C.bases); C.n_blocks = (uint32_t)R.bases.size();
     CU(cudaMalloc(&C.rep, 24)); C.allocs.push_back(C.rep);
+    // a cudaMemcpy from pageable memory may return before its DMA is done, and the first reader may be a non-blocking stream
+    CU(cudaStreamSynchronize(0));
     C.ready = true;
     return C;
 }
@@ -1081,7 +1101,7 @@ static bool misaligned16(std::initializer_list<const void *> bufs) {
 int pob_r1cs_products(pob_handle *h, uint32_t index, uint64_t first_row, uint64_t n_rows, void *a, void *b, void *c, void *consumer_stream) {
     if (!h) return fail(POB_E_BAD_ARG, "pob_r1cs_products: null handle");
     if (misaligned16({a, b, c})) return fail(POB_E_BAD_ARG, "pob_r1cs_products: a, b and c must be 16-byte aligned");
-    uint64_t *s = nullptr; int rc = resident_slot(h, index, &s); if (rc) return rc;
+    uint64_t *s = nullptr; int rc = resident_slot(h, index, &s, (cudaStream_t)consumer_stream); if (rc) return rc;
     try {
         CU(cudaSetDevice(h->device));
         pob_handle::DevCons &C = ensure_r1cs(h);
@@ -1116,6 +1136,7 @@ static const NttTables &ensure_ntt(pob_handle *h, uint32_t L) {
     N.t.w_lo = up(H.w_lo); N.t.w_hi = up(H.w_hi); N.t.loc = up(H.loc); N.t.loc_inv = up(H.loc_inv);
     N.t.g_lo = up(H.g_lo); N.t.g_hi = up(H.g_hi); N.t.g_log = H.g_log;
     CU(ntt_init_kernels());
+    CU(cudaStreamSynchronize(0));                      // the uploads are done before a consumer stream reads them (ensure_r1cs)
     N.log_n = L; N.ready = true;
     return N.t;
 }
@@ -1132,7 +1153,7 @@ int pob_r1cs_domain(pob_handle *h, uint32_t *log_n) {
 int pob_r1cs_quotient(pob_handle *h, uint32_t index, void *out, void *work, void *consumer_stream) {
     if (!h || !out || !work) return fail(POB_E_BAD_ARG, "pob_r1cs_quotient: null argument");
     if (misaligned16({out, work})) return fail(POB_E_BAD_ARG, "pob_r1cs_quotient: out and work must be 16-byte aligned");
-    uint64_t *s = nullptr; int rc = resident_slot(h, index, &s); if (rc) return rc;
+    uint64_t *s = nullptr; int rc = resident_slot(h, index, &s, (cudaStream_t)consumer_stream); if (rc) return rc;
     try {
         CU(cudaSetDevice(h->device));
         pob_handle::DevCons &C = ensure_r1cs(h);
