@@ -348,10 +348,8 @@ __global__ void __maxnreg__(THREADS == 1024 ? 64 : 104) k_eval(const EvalArgs a)
 
 // Half a 32-byte entry as one 128-bit store (STG.E.128; sm_90 has no 256-bit store).  No "memory" clobber on purpose: the
 // compiler must be free to hoist the next entries' loads above it so that several loads are in flight per thread (the
-// witness is written, never read, here).  The streaming flavour is evict-first in L2, so that the witness write stream does
-// not flush the eval kernel's working set out of L2.
+// witness is written, never read, here).
 __device__ __forceinline__ void st128(uint64_t *p, uint64_t a, uint64_t b) { asm volatile("st.global.v2.b64 [%0], {%1, %2};" ::"l"(p), "l"(a), "l"(b)); }
-__device__ __forceinline__ void st128cs(uint64_t *p, uint64_t a, uint64_t b) { asm volatile("st.global.cs.v2.b64 [%0], {%1, %2};" ::"l"(p), "l"(a), "l"(b)); }
 
 struct ExpandArgs {
     const Tile *tiles; const Code *codes; const Fr *konst; const uint2 *round_desc;
@@ -361,15 +359,14 @@ struct ExpandArgs {
     const uint32_t *status;                       // per instance of the batch; a rejected instance contributes no witness
     uint32_t chunk_first;                         // batch index of the chunk's first instance (store = inst - chunk_first)
     uint32_t tile0;                               // first tile of this launch (k_expand_codes)
-    uint32_t cs;                                  // 1: streaming (evict-first) witness stores
 };
 
 // k_expand_round: grid = (KeccakfRound tiles, instances in the group) -- 95.8 % of the witness.  One CTA streams one
 // tile (<= 4096 entries = 128 KiB in the O0 layout) with one 128-bit store per half entry.  The source of every entry
 // follows from an 8-byte descriptor per 64 entries and a lane word of the round; the tile's <= 130 descriptors and the round's 263 words are
 // staged in shared memory by two TMA bulk copies, so the streaming loop touches no global memory but the witness itself.
-template <int T>
-__global__ void __launch_bounds__(T) k_expand_round(const ExpandArgs a) {
+constexpr int ROUND_THREADS = 256;
+__global__ void __launch_bounds__(ROUND_THREADS) k_expand_round(const ExpandArgs a) {
     const uint32_t gi = a.inst[blockIdx.y];
     if (a.status[gi] != 0) return;                // reference: a failed assert leaves no witness (tests/test.py:65-68)
     const Tile t = a.tiles[blockIdx.x];
@@ -395,7 +392,7 @@ __global__ void __launch_bounds__(T) k_expand_round(const ExpandArgs a) {
     // covers 512 contiguous bytes.  Two 128-bit stores of the same thread per entry would leave every store instruction
     // half of each 32-byte sector it touches, twice the L2 write requests for the same bytes.
 #pragma unroll 8
-    for (uint32_t u = threadIdx.x; u < 2 * t.n; u += T) {
+    for (uint32_t u = threadIdx.x; u < 2 * t.n; u += ROUND_THREADS) {
         const uint32_t k = u >> 1;
         const uint2 d = sD[k >> 6];
         const uint32_t tt = k & 63, mode = d.y >> 16;
@@ -405,7 +402,7 @@ __global__ void __launch_bounds__(T) k_expand_round(const ExpandArgs a) {
             b = g; w = (m == 0) ? (d.x & 0xffffu) : (m == 1) ? (d.x >> 16) : (d.y & 0xffffu);
         }
         const uint64_t v = (u & 1u) ? 0ull : (sW[w] >> b) & 1ull;
-        if (a.cs) st128cs(W + 2ull * u, v, 0); else st128(W + 2ull * u, v, 0);
+        st128(W + 2ull * u, v, 0);
     }
 }
 
@@ -451,7 +448,7 @@ __global__ void __launch_bounds__(256, 3) k_expand_codes(const ExpandArgs a) {
             } else if (!h) v[j][0] = (kind == K_BIT) ? (Ub[p >> 6] >> (p & 63)) & 1ull : p;
         }
 #pragma unroll
-        for (int j = 0; j < UG; j++) { const uint32_t u = base + 256 * j; if (u < n2) { if (a.cs) st128cs(W + 2ull * u, v[j][0], v[j][1]); else st128(W + 2ull * u, v[j][0], v[j][1]); } }
+        for (int j = 0; j < UG; j++) { const uint32_t u = base + 256 * j; if (u < n2) st128(W + 2ull * u, v[j][0], v[j][1]); }
     }
 }
 

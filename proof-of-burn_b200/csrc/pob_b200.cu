@@ -201,19 +201,17 @@ struct pob_handle {
     // k_expand_codes likewise carries 24 KiB next to its 32 KiB code buffer: THREE resident CTAs per SM instead of six.  With
     // half-entry stores the code tiles take 68 instead of 85 ms per 512 witnesses that way (H100, DESIGN.md §2.3)
     uint32_t codes_dyn_smem = 24 * 1024;
-    uint32_t round_threads = 256, codes_overlap = 0; bool serialize = false;   // changed by POB_TUNING knobs only
     int eval_threads = 512; uint32_t eval_cluster = 0, eval_prefetch = 0;   // k_eval: threads per CTA; CTAs per instance (0 = chosen per launch)
     uint32_t pos_konst_bytes = 0, levels_bytes = 0, eval_smem = 0;
     bool skip_eval = false;                     // tuning: evaluate only the first two chunks, then re-expand their stores (isolates the cost of concurrency)
-    uint32_t expand_cs = 0, eval_l2_mb = 0;     // tuning: streaming witness stores; persisting-L2 window (MB) for the eval stream's store accesses
-    cudaStream_t s_eval = nullptr, s_exp = nullptr, s_exp2 = nullptr, s_h2d = nullptr;
+    cudaStream_t s_eval = nullptr, s_exp = nullptr, s_h2d = nullptr;
     cudaEvent_t ev_eval_done[RING] = {nullptr, nullptr}, ev_exp_done[RING] = {nullptr, nullptr}, ev_h2d[RING] = {nullptr, nullptr},
-                ev_start = nullptr, ev_end = nullptr, ev_tmp = nullptr, ev_fork = nullptr, ev_join = nullptr;
+                ev_start = nullptr, ev_end = nullptr, ev_tmp = nullptr;
     std::vector<cudaEvent_t> ev_pool; size_t ev_used = 0;
     // the batch in flight
     struct Group { uint32_t begin, end, chunk; cudaEvent_t t0, t1; };
     struct Batch {
-        bool active = false, async = false, staged = false, expand = false, digest = false;
+        bool active = false, async = false, staged = false, digest = false;
         const uint64_t *inputs = nullptr; uint32_t n = 0, nchunks = 0, next_eval = 0, next_group = 0, acq_pos = 0;
         std::vector<uint32_t> plan, slot;         // instances to materialise (ascending) and their slots
         std::vector<uint8_t> st;                  // per plan entry: 0 = not handed out yet, 1 = held by the consumer, 2 = released / dropped
@@ -366,31 +364,18 @@ static void enqueue_group(pob_handle *h, uint32_t g) {
         h->slot_owner[s] = (int64_t)B.plan[k];
     }
     ExpandArgs xa{h->d_tiles, h->d_codes, h->d_konst, reinterpret_cast<const uint2 *>(h->d_round_desc), h->d_stores + (size_t)r * E * h->store_stride, h->store_stride, P.val_base,
-                  h->d_witptr + G.begin, h->d_planinst + G.begin, h->d_status, G.chunk * E, 0, h->expand_cs};
+                  h->d_witptr + G.begin, h->d_planinst + G.begin, h->d_status, G.chunk * E, 0};
     CU(cudaEventRecord(G.t0, h->s_exp));
     // launch 1: KeccakfRound tiles, tile-major (each CTA's tables are staged in shared memory);
     // launch 2: code tiles, INSTANCE-major, so that a tile's code stream is fetched from DRAM once and
     // served from L2 to the other witnesses of the group
-    // codes_overlap: the code-tile kernel (gathers from the instance store) runs on a second stream NEXT TO the round kernel (bandwidth-bound)
-    // instead of after it; 1 = round kernel launched first, 2 = code kernel launched first
     const uint32_t n_round = h->n_round_tiles, n_code = (uint32_t)P.tiles.size() - n_round;
-    const bool fork = h->codes_overlap && n_round && n_code;
-    cudaStream_t s_codes = fork ? h->s_exp2 : h->s_exp;
-    auto launch_codes = [&]() {
+    if (n_round) k_expand_round<<<dim3(n_round, gc), ROUND_THREADS, h->round_dyn_smem, h->s_exp>>>(xa);
+    if (n_code) {
         xa.tile0 = n_round;
-        k_expand_codes<<<dim3(gc, n_code), 256, h->codes_dyn_smem, s_codes>>>(xa);
+        k_expand_codes<<<dim3(gc, n_code), 256, h->codes_dyn_smem, h->s_exp>>>(xa);
         B.T.other_launches++;
-    };
-    if (fork) { CU(cudaEventRecord(h->ev_fork, h->s_exp)); CU(cudaStreamWaitEvent(h->s_exp2, h->ev_fork, 0)); if (h->codes_overlap == 2) launch_codes(); }
-    if (n_round) {
-        xa.tile0 = 0;
-        if (h->round_threads == 128) k_expand_round<128><<<dim3(n_round, gc), 128, h->round_dyn_smem, h->s_exp>>>(xa);
-        else if (h->round_threads == 512) k_expand_round<512><<<dim3(n_round, gc), 512, h->round_dyn_smem, h->s_exp>>>(xa);
-        else if (h->round_threads == 1024) k_expand_round<1024><<<dim3(n_round, gc), 1024, h->round_dyn_smem, h->s_exp>>>(xa);
-        else k_expand_round<256><<<dim3(n_round, gc), 256, h->round_dyn_smem, h->s_exp>>>(xa);
     }
-    if (n_code && !(fork && h->codes_overlap == 2)) launch_codes();
-    if (fork) { CU(cudaEventRecord(h->ev_join, h->s_exp2)); CU(cudaStreamWaitEvent(h->s_exp, h->ev_join, 0)); }
     CU(cudaEventRecord(G.t1, h->s_exp));
     B.T.expand_launches++;
     if (B.digest) for (uint32_t k = G.begin; k < G.end; k++) {     // built-in on-GPU consumer: reads every entry of the witness once
@@ -398,10 +383,7 @@ static void enqueue_group(pob_handle *h, uint32_t g) {
         B.T.other_launches++;
     }
     if (!B.async) for (uint32_t k = G.begin; k < G.end; k++) B.st[k] = 2;   // synchronous batch: consumed by the digest (same stream) or dropped on request
-    if (g + 1 == B.chunk_gend[G.chunk]) {
-        CU(cudaEventRecord(h->ev_exp_done[r], h->s_exp));
-        if (h->serialize) CU(cudaStreamWaitEvent(h->s_eval, h->ev_exp_done[r], 0));
-    }
+    if (g + 1 == B.chunk_gend[G.chunk]) CU(cudaEventRecord(h->ev_exp_done[r], h->s_exp));
 }
 
 static bool group_slots_free(const pob_handle *h, uint32_t g) {
@@ -436,7 +418,7 @@ static int begin_batch(pob_handle *h, const uint64_t *inputs, uint32_t n, uint32
     ensure_batch_buffers(h, n);
     pob_handle::Batch &B = h->B;
     B = pob_handle::Batch();
-    B.async = async; B.staged = staged; B.expand = expand; B.digest = digest; B.inputs = inputs; B.n = n;
+    B.async = async; B.staged = staged; B.digest = digest; B.inputs = inputs; B.n = n;
     const uint32_t E = h->chunk;
     B.nchunks = (n + E - 1) / E;
     // with a consumer in the loop two groups must fit the slot ring, else generation and consumption cannot overlap
@@ -462,7 +444,7 @@ static int begin_batch(pob_handle *h, const uint64_t *inputs, uint32_t n, uint32
     B.e0.resize(B.nchunks); B.e1.resize(B.nchunks); B.est.resize(B.nchunks);
     for (uint32_t c = 0; c < B.nchunks; c++) { B.e0[c] = pool_event(h); B.e1[c] = pool_event(h); B.est[c] = pool_event(h); }
     // the previous batch's residency ends here: its slots are about to be reused, but not before the consumer work its
-    // stream-ordered releases stand for (s_exp2 forks from s_exp, so it follows)
+    // stream-ordered releases stand for
     std::fill(h->slot_owner.begin(), h->slot_owner.end(), (int64_t)-1);
     for (size_t s = 0; s < h->slots.size(); s++)
         if (h->slot_rel_pending[s]) { CU(cudaStreamWaitEvent(h->s_exp, h->slot_rel_ev[s], 0)); h->slot_rel_pending[s] = 0; }
@@ -577,7 +559,6 @@ void pob_destroy(pob_handle *h) {
     for (void *p : h->r1cs.allocs) cudaFree(p);
     for (void *p : h->ntt.allocs) cudaFree(p);
     if (h->s_eval) cudaStreamSynchronize(h->s_eval);
-    if (h->s_exp2) cudaStreamSynchronize(h->s_exp2);
     if (h->s_exp) cudaStreamSynchronize(h->s_exp);
     if (h->s_h2d) cudaStreamSynchronize(h->s_h2d);
     for (void *p : {(void *)h->d_ops, (void *)h->d_psums, (void *)h->d_pos, (void *)h->d_pos_konst, (void *)h->d_abs, (void *)h->d_levels, (void *)h->d_aux, (void *)h->d_konst, (void *)h->d_codes,
@@ -601,8 +582,8 @@ void pob_destroy(pob_handle *h) {
         if (h->ev_exp_done[r]) cudaEventDestroy(h->ev_exp_done[r]);
         if (h->ev_h2d[r]) cudaEventDestroy(h->ev_h2d[r]);
     }
-    for (cudaEvent_t e : {h->ev_start, h->ev_end, h->ev_tmp, h->ev_fork, h->ev_join}) if (e) cudaEventDestroy(e);
-    for (cudaStream_t s : {h->s_h2d, h->s_eval, h->s_exp, h->s_exp2}) if (s) cudaStreamDestroy(s);
+    for (cudaEvent_t e : {h->ev_start, h->ev_end, h->ev_tmp}) if (e) cudaEventDestroy(e);
+    for (cudaStream_t s : {h->s_h2d, h->s_eval, h->s_exp}) if (s) cudaStreamDestroy(s);
     delete h;
 }
 
@@ -639,14 +620,12 @@ int pob_create(const char *main_name, const uint64_t *params, int nparams, int h
         CU(cudaStreamCreateWithPriority(&h->s_eval, cudaStreamNonBlocking, pr_greatest));
         CU(cudaStreamCreateWithPriority(&h->s_h2d, cudaStreamNonBlocking, pr_greatest));
         CU(cudaStreamCreateWithPriority(&h->s_exp, cudaStreamNonBlocking, pr_least));
-        CU(cudaStreamCreateWithPriority(&h->s_exp2, cudaStreamNonBlocking, pr_least));
         for (uint32_t r = 0; r < pob_handle::RING; r++) {
             CU(cudaEventCreateWithFlags(&h->ev_eval_done[r], cudaEventDisableTiming));
             CU(cudaEventCreateWithFlags(&h->ev_exp_done[r], cudaEventDisableTiming));
             CU(cudaEventCreateWithFlags(&h->ev_h2d[r], cudaEventDisableTiming));
         }
         CU(cudaEventCreate(&h->ev_start)); CU(cudaEventCreate(&h->ev_end)); CU(cudaEventCreateWithFlags(&h->ev_tmp, cudaEventDisableTiming));
-        CU(cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming)); CU(cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming));
         if (const char *v = tune_env("POB_EVAL_PROFILE")) { h->prof_path = v; CU(cudaMalloc(&h->d_prof, (P.levels.size() + 3) * sizeof(long long))); }
         // witness slots: as many as fit in 80 % of free HBM after the store ring
         size_t free_b = 0, total_b = 0; CU(cudaMemGetInfo(&free_b, &total_b));
@@ -702,39 +681,18 @@ int pob_create(const char *main_name, const uint64_t *params, int nparams, int h
         if (const char *v = tune_env("POB_EVAL_CLUSTER")) h->eval_cluster = (uint32_t)std::max(0, std::min(8, atoi(v)));
         if (const char *v = tune_env("POB_EVAL_PREFETCH")) h->eval_prefetch = (uint32_t)(atoi(v) != 0);
         if (const char *v = tune_env("POB_SKIP_EVAL")) h->skip_eval = atoi(v) != 0;
-        if (const char *v = tune_env("POB_EXPAND_CS")) h->expand_cs = (uint32_t)(atoi(v) != 0);
-        if (const char *v = tune_env("POB_EVAL_L2_MB")) h->eval_l2_mb = (uint32_t)std::max(0, atoi(v));
         if (h->eval_threads != 256 && h->eval_threads != 512) h->eval_threads = 1024;
         h->eval_smem = h->pos_konst_bytes + h->levels_bytes + INV_WORKERS * INV_PARK_WORDS * 4u;   // + the parked inversion state of 256 workers (33 KB)
         if (h->eval_smem > 200 * 1024) throw std::runtime_error("the Poseidon constant table, the level table and the parked inversions do not fit in shared memory");
         CU(cudaFuncSetAttribute(k_eval<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->eval_smem));
         CU(cudaFuncSetAttribute(k_eval<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->eval_smem));
         CU(cudaFuncSetAttribute(k_eval<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->eval_smem));
-        if (const char *v = tune_env("POB_SERIALIZE")) h->serialize = atoi(v) != 0;
         if (const char *v = tune_env("POB_EXPAND_SMEM_KB")) h->round_dyn_smem = (uint32_t)atoi(v) * 1024u;
-        if (const char *v = tune_env("POB_EXPAND_THREADS")) h->round_threads = (uint32_t)atoi(v);
-        if (const char *v = tune_env("POB_CODES_OVERLAP")) h->codes_overlap = (uint32_t)atoi(v);
         if (const char *v = tune_env("POB_CODES_SMEM_KB")) h->codes_dyn_smem = (uint32_t)atoi(v) * 1024u;
         // static (the 32 KiB code buffer) + dynamic shared memory above 48 KiB needs the opt-in
         CU(cudaFuncSetAttribute(k_expand_codes, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->codes_dyn_smem));
-        if (h->round_dyn_smem > 48 * 1024) {
-            CU(cudaFuncSetAttribute(k_expand_round<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->round_dyn_smem));
-            CU(cudaFuncSetAttribute(k_expand_round<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->round_dyn_smem));
-            CU(cudaFuncSetAttribute(k_expand_round<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->round_dyn_smem));
-            CU(cudaFuncSetAttribute(k_expand_round<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->round_dyn_smem));
-        }
+        if (h->round_dyn_smem > 48 * 1024) CU(cudaFuncSetAttribute(k_expand_round, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->round_dyn_smem));
         if (const char *v = tune_env("POB_EXPAND_GROUP")) h->xgroup = (uint32_t)std::max(1, std::min<int>(atoi(v), (int)std::min<uint64_t>(nslots, chunk)));
-        if (h->eval_l2_mb) {       // tuning: keep (part of) the store ring persisting in L2 for the kernels of the eval stream
-            const size_t ring = (size_t)pob_handle::RING * chunk * h->store_stride * 8, carve = (size_t)h->eval_l2_mb << 20;
-            CU(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, carve));
-            cudaDeviceProp prop; CU(cudaGetDeviceProperties(&prop, device));
-            cudaStreamAttrValue av{};
-            av.accessPolicyWindow.base_ptr = h->d_stores;
-            av.accessPolicyWindow.num_bytes = std::min<size_t>(ring, (size_t)prop.accessPolicyMaxWindowSize);
-            av.accessPolicyWindow.hitRatio = (float)std::min(1.0, (double)carve / (double)av.accessPolicyWindow.num_bytes);
-            av.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting; av.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-            CU(cudaStreamSetAttribute(h->s_eval, cudaStreamAttributeAccessPolicyWindow, &av));
-        }
         h->slot_owner.assign(nslots, -1); h->slot_rel_pending.assign(nslots, 0);
         for (uint64_t s = 0; s < nslots; s++) { cudaEvent_t e; CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); h->slot_rel_ev.push_back(e); }
     } catch (const std::exception &e) {
