@@ -267,6 +267,25 @@ int pob_r1cs_domain(pob_handle *h, uint32_t *log_n);
  * wait, nothing allocated).  The first call builds the root and coset tables (at most 2 MB), freed by pob_destroy. */
 int pob_r1cs_quotient(pob_handle *h, uint32_t index, void *out, void *work, void *consumer_stream);
 
+/* ---- the third stage: BN254 G1 multi-exponentiation (the prover's A, B1, C and H MSMs) ---------------------------------------
+ * out = sum_i [s_i] P_i over BN254 G1 (y^2 = x^3 + 3 over F_q, q = 0x30644e72...fd47, cofactor 1).
+ * bases  : n affine points, 64 B each: x then y, each a 32-byte LE element of F_q in MONTGOMERY form (R = 2^256), the form a
+ *          snarkjs .zkey stores its G1 sections in (as far as known here; not checked against a real .zkey).  (0, 0) = infinity.
+ *          Bases are not checked to be on the curve.
+ * scalars: n x 32 B LE integers, e.g. the resident witness (from pob_acquire) or q from pob_r1cs_quotient.  Any 256-bit
+ *          value is allowed; since every point has order r, [s]P = [s mod r]P.
+ * out    : one point, 64 B, x then y as CANONICAL 32-byte LE F_q elements; (0, 0) = infinity.  Device memory.
+ * work   : caller scratch of at least pob_msm_g1_work_bytes(n) bytes, not overlapping bases, scalars or out; at most 64 n bytes
+ *          for n >= 2^18 (the size of pob_r1cs_quotient's work, so the H MSM can reuse it).
+ * consumer_stream: NULL = return when done; else (a cudaStream_t) enqueued with no host wait and nothing allocated.
+ * n == 0, a null or non-16-byte-aligned pointer, a short or overlapping work, out overlapping bases or scalars: POB_E_BAD_ARG
+ * before anything is enqueued.  n > 2^31: POB_E_RANGE.  No such device: POB_E_NO_DEVICE.
+ * A Groth16 prover calls it four times: A over (A bases, w, n_signals), B1 likewise, C over (C bases, w + 32 (n_outputs + 1),
+ * n_signals - n_outputs - 1), H over (H bases, q, 2^log_n) (INTEGRATION.md §3(e)). */
+int pob_msm_g1_work_bytes(uint64_t n, uint64_t *bytes);          /* host-only, no GPU needed */
+int pob_msm_g1(int device, const void *bases, const void *scalars, uint64_t n,
+               void *out, void *work, uint64_t work_bytes, void *consumer_stream);
+
 /* ---- the step just before the path (SURVEY.md 8(f) rank 3) ------------------------------------------------------
  * replaces: find_burn_key() of the reference input generator (tests/main.py:47-56): starting at start_key, find the
  * first burnKey >= start_key whose keccak256(burnKey[32 BE] | revealAmount[32 BE] | burnExtraCommitment[32 BE] |

@@ -36,31 +36,40 @@ POB_HD uint32_t fr_r2_limb(int i) {
     return R2[i];
 }
 
+// The modulus-dependent operations below (geq_mod, mod_add, mod_sub, mont_mul) are templates over a modulus M -- M::limb(i), its
+// 32-bit limbs, and M::n0 = -M^-1 mod 2^32 -- and an element type T of eight 32-bit limbs `l`.  Their bounds hold for any odd
+// modulus below 2^254.  Fr is the instance FrMod; fq_hd.h adds F_q, the base field of BN254 G1 (the multi-exponentiation).
+struct FrMod {
+    static POB_HD uint32_t limb(int i) { return fr_p_limb(i); }
+    static constexpr uint32_t n0 = POB_N0;
+};
+
 POB_HD Fr fr_zero() { Fr r; for (int i = 0; i < 8; i++) r.l[i] = 0; return r; }
 POB_HD Fr fr_from_u64(uint64_t v) { Fr r = fr_zero(); r.l[0] = (uint32_t)v; r.l[1] = (uint32_t)(v >> 32); return r; }
 POB_HD bool fr_is_zero(const Fr &a) { uint32_t o = 0; for (int i = 0; i < 8; i++) o |= a.l[i]; return o == 0; }
 POB_HD bool fr_eq(const Fr &a, const Fr &b) { uint32_t o = 0; for (int i = 0; i < 8; i++) o |= a.l[i] ^ b.l[i]; return o == 0; }
 POB_HD bool fr_fits64(const Fr &a) { uint32_t o = 0; for (int i = 2; i < 8; i++) o |= a.l[i]; return o == 0; }
 POB_HD uint64_t fr_lo64(const Fr &a) { return (uint64_t)a.l[0] | ((uint64_t)a.l[1] << 32); }
-// a >= p ?
-POB_HD bool fr_geq_p(const Fr &a) {
+// a >= M ?
+template <class M, class T> POB_HD bool geq_mod(const T &a) {
 #ifdef __CUDA_ARCH__
-    uint32_t br;                                                       // borrow of a - p
+    uint32_t br;                                                       // borrow of a - M
     asm("sub.cc.u32 %0, %1, %9;\n\tsubc.cc.u32 %0, %2, %10;\n\tsubc.cc.u32 %0, %3, %11;\n\tsubc.cc.u32 %0, %4, %12;\n\t"
         "subc.cc.u32 %0, %5, %13;\n\tsubc.cc.u32 %0, %6, %14;\n\tsubc.cc.u32 %0, %7, %15;\n\tsubc.cc.u32 %0, %8, %16;\n\t"
         "subc.u32 %0, 0, 0;"
         : "=&r"(br)
         : "r"(a.l[0]), "r"(a.l[1]), "r"(a.l[2]), "r"(a.l[3]), "r"(a.l[4]), "r"(a.l[5]), "r"(a.l[6]), "r"(a.l[7]),
-          "r"(fr_p_limb(0)), "r"(fr_p_limb(1)), "r"(fr_p_limb(2)), "r"(fr_p_limb(3)), "r"(fr_p_limb(4)), "r"(fr_p_limb(5)), "r"(fr_p_limb(6)), "r"(fr_p_limb(7)));
+          "r"(M::limb(0)), "r"(M::limb(1)), "r"(M::limb(2)), "r"(M::limb(3)), "r"(M::limb(4)), "r"(M::limb(5)), "r"(M::limb(6)), "r"(M::limb(7)));
     return br == 0;
 #else
-    for (int i = 7; i >= 0; i--) { uint32_t p = fr_p_limb(i); if (a.l[i] > p) return true; if (a.l[i] < p) return false; }
+    for (int i = 7; i >= 0; i--) { uint32_t p = M::limb(i); if (a.l[i] > p) return true; if (a.l[i] < p) return false; }
     return true;
 #endif
 }
+POB_HD bool fr_geq_p(const Fr &a) { return geq_mod<FrMod>(a); }
 // r = a + b / a - b mod 2^256, returning the carry / borrow.  On the device one carry chain (add.cc / addc.cc): the portable form
 // costs four instructions per limb.
-POB_HD uint32_t fr_raw_add(Fr &r, const Fr &a, const Fr &b) {
+template <class T> POB_HD uint32_t raw_add(T &r, const T &a, const T &b) {
 #ifdef __CUDA_ARCH__
     uint32_t c;
     asm("add.cc.u32 %0, %9, %17;\n\taddc.cc.u32 %1, %10, %18;\n\taddc.cc.u32 %2, %11, %19;\n\taddc.cc.u32 %3, %12, %20;\n\t"
@@ -76,7 +85,7 @@ POB_HD uint32_t fr_raw_add(Fr &r, const Fr &a, const Fr &b) {
     return (uint32_t)c;
 #endif
 }
-POB_HD uint32_t fr_raw_sub(Fr &r, const Fr &a, const Fr &b) {
+template <class T> POB_HD uint32_t raw_sub(T &r, const T &a, const T &b) {
 #ifdef __CUDA_ARCH__
     uint32_t br;
     asm("sub.cc.u32 %0, %9, %17;\n\tsubc.cc.u32 %1, %10, %18;\n\tsubc.cc.u32 %2, %11, %19;\n\tsubc.cc.u32 %3, %12, %20;\n\t"
@@ -92,35 +101,40 @@ POB_HD uint32_t fr_raw_sub(Fr &r, const Fr &a, const Fr &b) {
     return (uint32_t)br;
 #endif
 }
-POB_HD Fr fr_p() { Fr r; for (int i = 0; i < 8; i++) r.l[i] = fr_p_limb(i); return r; }
-POB_HD Fr fr_add(const Fr &a, const Fr &b) {
+POB_HD uint32_t fr_raw_add(Fr &r, const Fr &a, const Fr &b) { return raw_add(r, a, b); }
+POB_HD uint32_t fr_raw_sub(Fr &r, const Fr &a, const Fr &b) { return raw_sub(r, a, b); }
+template <class M, class T> POB_HD T mod_value() { T r; for (int i = 0; i < 8; i++) r.l[i] = M::limb(i); return r; }
+POB_HD Fr fr_p() { return mod_value<FrMod, Fr>(); }
+template <class M, class T> POB_HD T mod_add(const T &a, const T &b) {
 #ifdef __CUDA_ARCH__
-    Fr r, t; fr_raw_add(r, a, b);                                     // a, b < p < 2^254: no carry out
-    const uint32_t keep = 0u - fr_raw_sub(t, r, fr_p());              // all-ones: r < p
+    T r, t; raw_add(r, a, b);                                          // a, b < M < 2^254: no carry out
+    const uint32_t keep = 0u - raw_sub(t, r, mod_value<M, T>());      // all-ones: r < M
 #pragma unroll
     for (int i = 0; i < 8; i++) t.l[i] ^= (t.l[i] ^ r.l[i]) & keep;
     return t;
 #else
-    Fr r; uint32_t c = fr_raw_add(r, a, b);
-    if (c || fr_geq_p(r)) { Fr t; fr_raw_sub(t, r, fr_p()); return t; }
+    T r; uint32_t c = raw_add(r, a, b);
+    if (c || geq_mod<M>(r)) { T t; raw_sub(t, r, mod_value<M, T>()); return t; }
     return r;
 #endif
 }
-POB_HD Fr fr_sub(const Fr &a, const Fr &b) {
+template <class M, class T> POB_HD T mod_sub(const T &a, const T &b) {
 #ifdef __CUDA_ARCH__
-    Fr r, t; const uint32_t wrap = 0u - fr_raw_sub(r, a, b);         // all-ones: a < b
-    fr_raw_add(t, r, fr_p());
+    T r, t; const uint32_t wrap = 0u - raw_sub(r, a, b);              // all-ones: a < b
+    raw_add(t, r, mod_value<M, T>());
 #pragma unroll
     for (int i = 0; i < 8; i++) r.l[i] ^= (r.l[i] ^ t.l[i]) & wrap;
     return r;
 #else
-    Fr r; if (fr_raw_sub(r, a, b)) { Fr t; fr_raw_add(t, r, fr_p()); return t; }
+    T r; if (raw_sub(r, a, b)) { T t; raw_add(t, r, mod_value<M, T>()); return t; }
     return r;
 #endif
 }
+POB_HD Fr fr_add(const Fr &a, const Fr &b) { return mod_add<FrMod>(a, b); }
+POB_HD Fr fr_sub(const Fr &a, const Fr &b) { return mod_sub<FrMod>(a, b); }
 POB_HD Fr fr_neg(const Fr &a) { if (fr_is_zero(a)) return a; Fr t; fr_raw_sub(t, fr_p(), a); return t; }
 
-// Montgomery product a*b*2^-256 mod p.  Result < p (one conditional subtraction); a < p, b < 2^256.
+// Montgomery product a*b*2^-256 mod M.  Result < M (one conditional subtraction); a < M, b < 2^256.
 // Portable form (host, emulator, `make portable`): column-wise (product scanning) -- the 64 limb products of the 512-bit product
 // are mutually independent (each column keeps a split lo/hi accumulator, so no carry chain links them), and the reduction needs
 // only the 8-step chain m_k = column_k * n0'.  On the device it compiles to 620 instructions (130 IMAD.WIDE + 354 adds).
@@ -130,8 +144,9 @@ POB_HD Fr fr_neg(const Fr &a) { if (fr_is_zero(a)) return a; Fr t; fr_raw_sub(t,
 // carry-in/out predicates -- 128 multiply-adds and ~70 other instructions per product instead of ~620 (the portable form below
 // splits every product into halves to keep its column sums inside 64 bits).  Per word b_i: E += a_even*b_i, O += a_odd*b_i,
 // m = E0*n0', E += p_even*m, O += p_odd*m, then t >>= 32 (E' = O, O' = E >> 64, E'[0] += E[1]) -- a renaming in unrolled code.
-// Bounds (a < p, b < 2^256): t < 2^288 before the shift, so E needs 9 limbs, O 8, and no O row carries out.  The algorithm
-// (same chains, same renaming) is checked against big-integer arithmetic by tests/test_host.py::test_even_odd_montgomery_model.
+// Bounds (a < M < 2^254, b < 2^256): t < 2^288 before the shift, so E needs 9 limbs, O 8, and no O row carries out.  The algorithm
+// (same chains, same renaming) is checked against big-integer arithmetic by tests/test_host.py::test_even_odd_montgomery_model,
+// and with the F_q modulus by tests/test_msm_cpu.py.
 #define POB_ROW(T, s0, s1, s2, s3, w)                                                                                              \
     "mad.lo.cc.u32 %0, %" s0 ", %" w ", %0;\n\tmadc.hi.cc.u32 %1, %" s0 ", %" w ", %1;\n\t"                                         \
     "madc.lo.cc.u32 %2, %" s1 ", %" w ", %2;\n\tmadc.hi.cc.u32 %3, %" s1 ", %" w ", %3;\n\t"                                        \
@@ -158,7 +173,7 @@ __device__ __forceinline__ void mont_row_o_carry(uint32_t &e0, uint32_t x, uint3
         : "+r"(T[0]), "+r"(T[1]), "+r"(T[2]), "+r"(T[3]), "+r"(T[4]), "+r"(T[5]), "+r"(T[6]), "+r"(T[7]), "+r"(e0)
         : "r"(s0), "r"(s1), "r"(s2), "r"(s3), "r"(w), "r"(x));
 }
-__device__ __forceinline__ Fr fr_mont(const Fr &a, const Fr &b) {
+template <class M, class T> __device__ __forceinline__ T mont_mul(const T &a, const T &b) {
     uint32_t E[9], O[9], x = 0;
 #pragma unroll
     for (int k = 0; k < 9; k++) E[k] = O[k] = 0;
@@ -167,9 +182,9 @@ __device__ __forceinline__ Fr fr_mont(const Fr &a, const Fr &b) {
         const uint32_t bi = b.l[i];
         mont_row_o_carry(E[0], x, O, a.l[1], a.l[3], a.l[5], a.l[7], bi);
         mont_row_e(E, a.l[0], a.l[2], a.l[4], a.l[6], bi);
-        const uint32_t m = E[0] * POB_N0;
-        mont_row_o(O, fr_p_limb(1), fr_p_limb(3), fr_p_limb(5), fr_p_limb(7), m);
-        mont_row_e(E, fr_p_limb(0), fr_p_limb(2), fr_p_limb(4), fr_p_limb(6), m);                    // E[0] is 0 now
+        const uint32_t m = E[0] * M::n0;
+        mont_row_o(O, M::limb(1), M::limb(3), M::limb(5), M::limb(7), m);
+        mont_row_e(E, M::limb(0), M::limb(2), M::limb(4), M::limb(6), m);                    // E[0] is 0 now
         x = E[1];
         uint32_t N[9];
 #pragma unroll
@@ -181,54 +196,55 @@ __device__ __forceinline__ Fr fr_mont(const Fr &a, const Fr &b) {
 #pragma unroll
         for (int k = 0; k < 9; k++) O[k] = N[k];
     }
-    Fr r;
+    T r;
     asm("add.cc.u32 %0, %8, %16;\n\taddc.cc.u32 %1, %9, %17;\n\taddc.cc.u32 %2, %10, %18;\n\taddc.cc.u32 %3, %11, %19;\n\t"
         "addc.cc.u32 %4, %12, %20;\n\taddc.cc.u32 %5, %13, %21;\n\taddc.cc.u32 %6, %14, %22;\n\taddc.u32 %7, %15, %23;"
         : "=r"(r.l[0]), "=r"(r.l[1]), "=r"(r.l[2]), "=r"(r.l[3]), "=r"(r.l[4]), "=r"(r.l[5]), "=r"(r.l[6]), "=r"(r.l[7])
         : "r"(E[0]), "r"(E[1]), "r"(E[2]), "r"(E[3]), "r"(E[4]), "r"(E[5]), "r"(E[6]), "r"(E[7]),
           "r"(x), "r"(O[0]), "r"(O[1]), "r"(O[2]), "r"(O[3]), "r"(O[4]), "r"(O[5]), "r"(O[6]));
-    if (fr_geq_p(r)) { Fr sub; fr_raw_sub(sub, r, fr_p()); return sub; }                               // r < 2p
+    if (geq_mod<M>(r)) { T sub; raw_sub(sub, r, mod_value<M, T>()); return sub; }                     // r < 2M
     return r;
 }
 #undef POB_ROW
 #else
-POB_HD Fr fr_mont(const Fr &a, const Fr &b) {
-    uint32_t T[16];
+template <class M, class T> POB_HD T mont_mul(const T &a, const T &b) {
+    uint32_t X[16];
     uint64_t c = 0;
 #pragma unroll
-    for (int k = 0; k < 15; k++) {                       // T = a * b
+    for (int k = 0; k < 15; k++) {                       // X = a * b
         uint64_t lo = c, hi = 0;
 #pragma unroll
         for (int i = 0; i < 8; i++) {
             const int jj = k - i;
             if (jj >= 0 && jj < 8) { const uint64_t p = (uint64_t)a.l[i] * b.l[jj]; lo += (uint32_t)p; hi += p >> 32; }
         }
-        T[k] = (uint32_t)lo; c = (lo >> 32) + hi;
+        X[k] = (uint32_t)lo; c = (lo >> 32) + hi;
     }
-    T[15] = (uint32_t)c;
+    X[15] = (uint32_t)c;
     uint32_t m[8];
     c = 0;
 #pragma unroll
     for (int k = 0; k < 8; k++) {                        // low half: choose m_k so that column k becomes 0 mod 2^32
-        uint64_t lo = c + T[k], hi = 0;
+        uint64_t lo = c + X[k], hi = 0;
 #pragma unroll
-        for (int i = 0; i < 8; i++) if (i < k) { const uint64_t p = (uint64_t)m[i] * fr_p_limb(k - i); lo += (uint32_t)p; hi += p >> 32; }
-        m[k] = (uint32_t)lo * POB_N0;
-        const uint64_t p0 = (uint64_t)m[k] * fr_p_limb(0); lo += (uint32_t)p0; hi += p0 >> 32;
+        for (int i = 0; i < 8; i++) if (i < k) { const uint64_t p = (uint64_t)m[i] * M::limb(k - i); lo += (uint32_t)p; hi += p >> 32; }
+        m[k] = (uint32_t)lo * M::n0;
+        const uint64_t p0 = (uint64_t)m[k] * M::limb(0); lo += (uint32_t)p0; hi += p0 >> 32;
         c = (lo >> 32) + hi;
     }
-    Fr r;
+    T r;
 #pragma unroll
     for (int k = 8; k < 16; k++) {                       // high half: the result limbs
-        uint64_t lo = c + T[k], hi = 0;
+        uint64_t lo = c + X[k], hi = 0;
 #pragma unroll
-        for (int i = 0; i < 8; i++) { const int jj = k - i; if (jj >= 1 && jj < 8) { const uint64_t p = (uint64_t)m[i] * fr_p_limb(jj); lo += (uint32_t)p; hi += p >> 32; } }
+        for (int i = 0; i < 8; i++) { const int jj = k - i; if (jj >= 1 && jj < 8) { const uint64_t p = (uint64_t)m[i] * M::limb(jj); lo += (uint32_t)p; hi += p >> 32; } }
         r.l[k - 8] = (uint32_t)lo; c = (lo >> 32) + hi;
     }
-    if (c || fr_geq_p(r)) { Fr sub; fr_raw_sub(sub, r, fr_p()); return sub; }
+    if (c || geq_mod<M>(r)) { T sub; raw_sub(sub, r, mod_value<M, T>()); return sub; }
     return r;
 }
 #endif
+POB_HD Fr fr_mont(const Fr &a, const Fr &b) { return mont_mul<FrMod>(a, b); }
 POB_HD Fr fr_r2() { Fr r; for (int i = 0; i < 8; i++) r.l[i] = fr_r2_limb(i); return r; }
 POB_HD Fr fr_to_mont(const Fr &a) { return fr_mont(a, fr_r2()); }
 POB_HD Fr fr_from_mont(const Fr &a) { Fr one = fr_from_u64(1); return fr_mont(a, one); }

@@ -27,6 +27,7 @@
 #include "../../include/pob_b200.h"
 #include "compiler.h"
 #include "kernels.cuh"
+#include "msm.cuh"
 #include "ntt.cuh"
 #include "r1cs.h"
 
@@ -1141,6 +1142,40 @@ int pob_r1cs_quotient(pob_handle *h, uint32_t index, void *out, void *work, void
         }
         if (!consumer_stream) CU(cudaStreamSynchronize(st));
     } catch (const std::exception &e) { return fail(POB_E_CUDA, std::string("pob_r1cs_quotient: ") + e.what()); }
+    return POB_OK;
+}
+
+// ---- the G1 multi-exponentiation (msm.cuh) -----------------------------------------------------------------------------
+int pob_msm_g1_work_bytes(uint64_t n, uint64_t *bytes) {
+    if (!bytes || n == 0) return fail(POB_E_BAD_ARG, "pob_msm_g1_work_bytes: null argument or n == 0");
+    if (n > MSM_MAX_N) return fail(POB_E_RANGE, "pob_msm_g1_work_bytes: n exceeds 2^31");
+    *bytes = msm_layout(n).bytes;
+    return POB_OK;
+}
+
+int pob_msm_g1(int device, const void *bases, const void *scalars, uint64_t n, void *out, void *work, uint64_t work_bytes, void *consumer_stream) {
+    if (!bases || !scalars || !out || !work || n == 0) return fail(POB_E_BAD_ARG, "pob_msm_g1: null argument or n == 0");
+    if (misaligned16({bases, scalars, out, work})) return fail(POB_E_BAD_ARG, "pob_msm_g1: bases, scalars, out and work must be 16-byte aligned");
+    if (n > MSM_MAX_N) return fail(POB_E_RANGE, "pob_msm_g1: n exceeds 2^31");
+    const uint64_t need = msm_layout(n).bytes;
+    if (work_bytes < need) return fail(POB_E_BAD_ARG, "pob_msm_g1: work is shorter than pob_msm_g1_work_bytes(n) = " + std::to_string(need));
+    auto overlap = [](const void *a, uint64_t na, const void *b, uint64_t nb) {
+        const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
+        return x < y + nb && y < x + na;
+    };
+    if (overlap(work, need, bases, 64 * n) || overlap(work, need, scalars, 32 * n) || overlap(work, need, out, 64))
+        return fail(POB_E_BAD_ARG, "pob_msm_g1: work overlaps bases, scalars or out");
+    if (overlap(out, 64, bases, 64 * n) || overlap(out, 64, scalars, 32 * n)) return fail(POB_E_BAD_ARG, "pob_msm_g1: out overlaps bases or scalars");
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) return fail(POB_E_NO_DEVICE, "pob_msm_g1: no such CUDA device");
+    try {
+        CU(cudaSetDevice(device));
+        int sms = 0;
+        CU(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+        const cudaStream_t st = (cudaStream_t)consumer_stream;
+        CU(msm_g1_enqueue((const uint4 *)bases, (const uint4 *)scalars, n, (uint4 *)out, (uint8_t *)work, (uint32_t)sms, st));
+        if (!consumer_stream) CU(cudaStreamSynchronize(st));
+    } catch (const std::exception &e) { return fail(POB_E_CUDA, std::string("pob_msm_g1: ") + e.what()); }
     return POB_OK;
 }
 

@@ -151,6 +151,10 @@ def lib():
         L.pob_r1cs_domain.argtypes = [vp, ctypes.POINTER(u32)]
         L.pob_r1cs_quotient.restype = ci
         L.pob_r1cs_quotient.argtypes = [vp, u32, vp, vp, vp]
+        L.pob_msm_g1_work_bytes.restype = ci
+        L.pob_msm_g1_work_bytes.argtypes = [u64, ctypes.POINTER(u64)]
+        L.pob_msm_g1.restype = ci
+        L.pob_msm_g1.argtypes = [ci, vp, vp, u64, vp, vp, u64, vp]
         L.pob_pow_grind.restype = ci
         L.pob_pow_grind.argtypes = [ci, vp, vp, vp, u32, u64, vp, ctypes.POINTER(u64)]
         L.pob_last_error.restype = ctypes.c_char_p
@@ -557,6 +561,47 @@ def pow_grind(start_key, reveal_amount, burn_extra_commitment, zero_bytes=2, max
     tries = ctypes.c_uint64(0)
     _check(lib().pob_pow_grind(int(device), a.ctypes.data, b.ctypes.data, c.ctypes.data, int(zero_bytes), int(max_tries), out.ctypes.data, ctypes.byref(tries)))
     return from_limbs(out[0]), int(tries.value)
+
+
+def msm_g1_work_bytes(n):
+    """bytes of scratch pob_msm_g1 needs for n points (host only, no GPU); at most 64 n for n >= 2^18"""
+    v = ctypes.c_uint64(0)
+    _check(lib().pob_msm_g1_work_bytes(int(n), ctypes.byref(v)))
+    return int(v.value)
+
+
+def msm_g1(bases, scalars, stream=None, out=None, work=None, device=None):
+    """sum_i [s_i] P_i over BN254 G1 on the GPU (pob_b200.h: pob_msm_g1).  bases: (n, 8) uint64 CUDA tensor, per point x then y as
+    Montgomery-form F_q limbs, (0, 0) = infinity.  scalars: (n, 4) uint64 CUDA tensor of 256-bit LE integers, or (device pointer, n)
+    for memory the caller owns, such as a resident witness (Circuit.acquire / witness_device_ptr).  Returns (x, y) as canonical
+    ints, or None for infinity.  With a stream (torch.cuda.Stream or raw cudaStream_t) the work and any out / work tensor it has
+    to allocate are enqueued on it, and the (8,) uint64 out tensor (x limbs, then y limbs) is returned unsynchronised."""
+    import torch
+    if isinstance(scalars, tuple):
+        s_ptr, n = int(scalars[0]), int(scalars[1])
+    else:
+        if scalars.dim() != 2 or scalars.shape[1] != 4 or scalars.dtype not in (torch.uint64, torch.int64) or not scalars.is_contiguous():
+            raise ValueError("msm_g1: scalars must be a contiguous (n, 4) uint64 tensor")
+        s_ptr, n = scalars.data_ptr(), scalars.shape[0]
+    if bases.dim() != 2 or bases.shape[1] != 8 or bases.shape[0] != n or bases.dtype not in (torch.uint64, torch.int64) or not bases.is_contiguous():
+        raise ValueError("msm_g1: bases must be a contiguous (n, 8) uint64 tensor with n = %d" % n)
+    dev = bases.device if device is None else torch.device("cuda", device)
+    handle = None if stream is None else getattr(stream, "cuda_stream", stream)
+    with torch.cuda.stream(torch.cuda.ExternalStream(handle, device=dev) if handle else torch.cuda.current_stream(dev)):
+        if out is None:
+            out = torch.empty(8, dtype=torch.uint64, device=dev)
+        if work is None:
+            work = torch.empty(msm_g1_work_bytes(n), dtype=torch.uint8, device=dev)
+    for t, what in ((bases, "bases"), (out, "out"), (work, "work")):
+        if not t.is_cuda or t.device != dev or not t.is_contiguous():
+            raise ValueError("msm_g1: %s must be a contiguous tensor on %s" % (what, dev))
+    _check(lib().pob_msm_g1(dev.index, bases.data_ptr(), s_ptr, n, out.data_ptr(), work.data_ptr(),
+                            work.numel() * work.element_size(), handle))
+    if handle:
+        return out
+    v = [int(x) & ((1 << 64) - 1) for x in out.cpu().tolist()]
+    x, y = (sum(v[4 * k + i] << (64 * i) for i in range(4)) for k in (0, 1))
+    return None if x == 0 and y == 0 else (x, y)
 
 
 def repad_pob_input(inp, max_layers, node_blocks, header_blocks):
