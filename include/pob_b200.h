@@ -286,6 +286,53 @@ int pob_msm_g1_work_bytes(uint64_t n, uint64_t *bytes);          /* host-only, n
 int pob_msm_g1(int device, const void *bases, const void *scalars, uint64_t n,
                void *out, void *work, uint64_t work_bytes, void *consumer_stream);
 
+/* ---- the fourth stage: BN254 G2 multi-exponentiation (the prover's B MSM) -------------------------------------------------------
+ * out = sum_i [s_i] P_i over BN254 G2: the twist y^2 = x^3 + 3 / (9 + u) over F_q2 = F_q[u] / (u^2 + 1), whose points of order r
+ * form a subgroup (the cofactor is not 1).  The same Pippenger pipeline as pob_msm_g1, over F_q2.
+ * bases  : n affine points, 128 B each: x.c0, x.c1, y.c0, y.c1 (x = x.c0 + x.c1 u), each a 32-byte LE element of F_q in MONTGOMERY
+ *          form, as the G1 bases (the form of a snarkjs .zkey's G2 sections as far as known here; not checked against a real .zkey).
+ *          All-zero = infinity.  Bases must lie in the order-r subgroup: this is NOT checked, and [s]P = [s mod r]P holds only there.
+ * scalars: n x 32 B LE integers, any 256-bit value (taken mod r).
+ * out    : one point, 128 B in the same order, CANONICAL F_q elements; all-zero = infinity.  Device memory.
+ * work   : caller scratch of at least pob_msm_g2_work_bytes(n) bytes, not overlapping bases, scalars or out.
+ * consumer_stream, argument checks and error codes: as pob_msm_g1. */
+int pob_msm_g2_work_bytes(uint64_t n, uint64_t *bytes);          /* host-only, no GPU needed */
+int pob_msm_g2(int device, const void *bases, const void *scalars, uint64_t n,
+               void *out, void *work, uint64_t work_bytes, void *consumer_stream);
+
+/* ---- the proof: Groth16 over BN254 from a resident witness and a proving key in device memory --------------------------------
+ * snarkjs's convention, which pob_r1cs_quotient follows: n_vars = pob_desc.n_signals of the handle's form, n_pub = n_outputs, the
+ * domain n = 2^log_n of pob_r1cs_domain.  w = resident witness `index`, q = its quotient (pob_r1cs_quotient).  The key is a set of
+ * device pointers to its sections (no .zkey is read here); every point is affine, Montgomery form, (0, 0) = infinity:
+ *   A  = alpha1 + sum_i w_i A_i  + [r] delta1
+ *   B  = beta2  + sum_i w_i B2_i + [s] delta2,   B1 = beta1 + sum_i w_i B1_i + [s] delta1
+ *   C  = sum_{i > n_pub} w_i C_i + sum_k q_k H_k + [s] A + [r] B1 - [r s] delta1
+ * r and s are any 256-bit values, taken mod r.  For zero knowledge they must be uniformly random and secret: that is the caller's
+ * job, this function draws no random numbers (r = s = 0 is accepted).  proof: 256 bytes of device memory, all canonical affine:
+ * A (64 B, x then y), B (128 B, x.c0, x.c1, y.c0, y.c1), C (64 B).
+ * The call enqueues on consumer_stream, with no host wait, nothing allocated and no host memory read after it returns (r and s go to
+ * the kernel by value): the quotient into `work`, the H MSM over it, the A, B1, C and B2 MSMs over the witness, one assembly kernel.
+ * Witness readiness and consumer_stream (NULL = return when done) are as pob_r1cs_quotient's, and so are the index errors.  A null
+ * argument, counts that differ from the handle's, a null or non-16-byte-aligned key pointer, proof or work, work shorter than
+ * pob_groth16_work_bytes, or a proof overlapping work: POB_E_BAD_ARG, before anything is enqueued. */
+typedef struct {
+    uint64_t n_vars;                       /* must equal the handle's n_signals  (else POB_E_BAD_ARG) */
+    uint32_t n_pub;                        /* must equal n_outputs               (else POB_E_BAD_ARG) */
+    uint32_t log_n;                        /* must equal pob_r1cs_domain         (else POB_E_BAD_ARG) */
+    const void *alpha1, *beta1, *delta1;   /* one G1 point each, 64 B, Montgomery, as pob_msm_g1 bases  */
+    const void *beta2, *delta2;            /* one G2 point each, 128 B, Montgomery, as pob_msm_g2 bases */
+    const void *a, *b1;                    /* n_vars G1 points                                           */
+    const void *b2;                        /* n_vars G2 points                                           */
+    const void *c;                         /* n_vars - n_pub - 1 G1 points, wires n_pub + 1 ..           */
+    const void *h;                         /* 2^log_n G1 points, paired with q[k] of pob_r1cs_quotient   */
+} pob_groth16_key;
+/* bytes of `work` a proof on this handle needs: q (32 n), then the largest of the quotient's 64 n and the MSM scratches, then the
+ * five MSM results (builds the row plan on first use, like pob_r1cs_domain) */
+int pob_groth16_work_bytes(pob_handle *h, uint64_t *bytes);
+int pob_groth16_prove(pob_handle *h, uint32_t index, const pob_groth16_key *key,
+                      const uint64_t r[4], const uint64_t s[4],
+                      void *proof, void *work, uint64_t work_bytes, void *consumer_stream);
+
 /* ---- the step just before the path (SURVEY.md 8(f) rank 3) ------------------------------------------------------
  * replaces: find_burn_key() of the reference input generator (tests/main.py:47-56): starting at start_key, find the
  * first burnKey >= start_key whose keccak256(burnKey[32 BE] | revealAmount[32 BE] | burnExtraCommitment[32 BE] |

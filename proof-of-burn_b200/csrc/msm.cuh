@@ -1,4 +1,6 @@
-// msm.cuh -- BN254 G1 multi-exponentiation sum_i [s_i] P_i (pob_msm_g1, DESIGN.md §5): Pippenger with signed c-bit digits.
+// msm.cuh -- BN254 multi-exponentiation sum_i [s_i] P_i over G1 (pob_msm_g1) or G2 (pob_msm_g2), DESIGN.md §5: Pippenger with
+// signed c-bit digits.  One pipeline for both groups: the kernels that carry points are templates over a curve trait (MsmCurve<F>,
+// F = Fq or Fq2: point types, formulas, loads and stores); k_msm_digits and k_msm_scan see only scalars and are shared.
 //
 // Per window j (one after another, so that the scratch holds one window's grouping):
 //   k_msm_digits<false>  signed digit d of every scalar (s mod r first); a histogram of |d| - 1 (the bucket).  d = 0 writes nothing.
@@ -19,7 +21,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <algorithm>
-#include "fq_hd.h"
+#include "fq2_hd.h"
 
 using namespace pob;
 
@@ -43,11 +45,23 @@ static uint32_t msm_window_bits(uint64_t n) {
 // chunks (threads) of the first bucket-sum level: about 16 grouped entries per thread for n <= 2^20, then at most 2^16 threads
 static uint32_t msm_chunks(uint64_t n) { return (uint32_t)std::min<uint64_t>(1u << 16, std::max<uint64_t>(32, n / 16)); }
 
+// a curve of the multi-exponentiation: points over F (G1: Fq, G2: Fq2), the formulas of fq_hd.h, and loads / stores of F as uint4s
+template <class F> struct MsmCurve {
+    typedef F Field;
+    typedef Aff<F> Affine;
+    typedef Xyzz<F> Point;
+    static const uint32_t FIELD_U4 = sizeof(F) / 16;                  // uint4s per element: 2 (Fq) or 4 (Fq2)
+    static const uint32_t AFF_BYTES = 2 * sizeof(F);                   // one affine base / output point
+};
+typedef MsmCurve<Fq> MsmG1;
+typedef MsmCurve<Fq2> MsmG2;
+
 struct MsmLayout {                        // byte offsets into the caller's work buffer
     uint32_t c, windows, buckets, chunks, seg_threads;
     uint64_t idx, cnt, offs, bkt, keys_a, pts_a, keys_b, pts_b, win, bytes;
 };
-static MsmLayout msm_layout(uint64_t n) {
+template <class C> static MsmLayout msm_layout(uint64_t n) {
+    typedef typename C::Point Pt;
     MsmLayout L;
     L.c = msm_window_bits(n);
     L.windows = (MSM_SCALAR_BITS + L.c - 1) / L.c;
@@ -61,12 +75,12 @@ static MsmLayout msm_layout(uint64_t n) {
     L.idx = take(4 * n);
     L.cnt = take(4ull * (L.buckets + 1));
     L.offs = take(4ull * (L.buckets + 1));
-    L.bkt = take(sizeof(G1Xyzz) * (uint64_t)L.buckets);
+    L.bkt = take(sizeof(Pt) * (uint64_t)L.buckets);
     L.keys_a = take(4 * pa);
-    L.pts_a = take(sizeof(G1Xyzz) * pa);
+    L.pts_a = take(sizeof(Pt) * pa);
     L.keys_b = take(4 * pb);
-    L.pts_b = take(sizeof(G1Xyzz) * pb);
-    L.win = take(sizeof(G1Xyzz) * (uint64_t)L.windows);
+    L.pts_b = take(sizeof(Pt) * pb);
+    L.win = take(sizeof(Pt) * (uint64_t)L.windows);
     L.bytes = at;
     return L;
 }
@@ -80,14 +94,20 @@ __device__ __forceinline__ void msm_st_fq(uint4 *p, const Fq &a) {
     p[0] = make_uint4(a.l[0], a.l[1], a.l[2], a.l[3]);
     p[1] = make_uint4(a.l[4], a.l[5], a.l[6], a.l[7]);
 }
-__device__ __forceinline__ G1Xyzz msm_ld_xyzz(const G1Xyzz *p) {
+__device__ __forceinline__ void msm_ld(const uint4 *p, Fq &r) { r = msm_ld_fq(p); }
+__device__ __forceinline__ void msm_ld(const uint4 *p, Fq2 &r) { r.c0 = msm_ld_fq(p); r.c1 = msm_ld_fq(p + 2); }
+__device__ __forceinline__ void msm_st(uint4 *p, const Fq &a) { msm_st_fq(p, a); }
+__device__ __forceinline__ void msm_st(uint4 *p, const Fq2 &a) { msm_st_fq(p, a.c0); msm_st_fq(p + 2, a.c1); }
+template <class F> __device__ __forceinline__ Xyzz<F> msm_ld_xyzz(const Xyzz<F> *p) {
     const uint4 *q = (const uint4 *)p;
-    G1Xyzz r; r.x = msm_ld_fq(q); r.y = msm_ld_fq(q + 2); r.zz = msm_ld_fq(q + 4); r.zzz = msm_ld_fq(q + 6);
+    const uint32_t u = MsmCurve<F>::FIELD_U4;
+    Xyzz<F> r; msm_ld(q, r.x); msm_ld(q + u, r.y); msm_ld(q + 2 * u, r.zz); msm_ld(q + 3 * u, r.zzz);
     return r;
 }
-__device__ __forceinline__ void msm_st_xyzz(G1Xyzz *p, const G1Xyzz &a) {
+template <class F> __device__ __forceinline__ void msm_st_xyzz(Xyzz<F> *p, const Xyzz<F> &a) {
     uint4 *q = (uint4 *)p;
-    msm_st_fq(q, a.x); msm_st_fq(q + 2, a.y); msm_st_fq(q + 4, a.zz); msm_st_fq(q + 6, a.zzz);
+    const uint32_t u = MsmCurve<F>::FIELD_U4;
+    msm_st(q, a.x); msm_st(q + u, a.y); msm_st(q + 2 * u, a.zz); msm_st(q + 3 * u, a.zzz);
 }
 
 // signed digit of window j of s mod r: s = sum_j d_j 2^(c j), d_j in (-2^(c-1), 2^(c-1)]
@@ -155,9 +175,10 @@ __global__ void __launch_bounds__(1024) k_msm_scan(uint32_t *cnt, uint32_t K, ui
 }
 
 // the entries of the first bucket-sum level: the grouped list of one window, keys from the bucket offsets
-struct MsmBases {
+template <class C> struct MsmBases {
+    typedef C Curve;
     const uint32_t *offs, *idx;
-    const uint4 *bases;                                                // n affine points, 4 x uint4 each
+    const uint4 *bases;                                                // n affine points, 2 FIELD_U4 uint4s each
     uint32_t K;
     __device__ uint32_t count() const { return offs[K]; }
     __device__ uint32_t first_key(uint32_t p) const {                  // the bucket b with offs[b] <= p < offs[b + 1]
@@ -166,23 +187,24 @@ struct MsmBases {
         return lo;
     }
     __device__ uint32_t next_key(uint32_t b, uint32_t p) const { while (offs[b + 1] <= p) b++; return b; }
-    __device__ void add(G1Xyzz &acc, uint32_t p) const {
+    __device__ void add(typename C::Point &acc, uint32_t p) const {
         const uint32_t e = __ldg(idx + p);
-        const uint4 *q = bases + 4 * (uint64_t)(e & 0x7fffffffu);
-        G1Aff a; a.x = msm_ld_fq(q); a.y = msm_ld_fq(q + 2);
-        if (e >> 31) a = g1_aff_neg(a);
-        acc = g1_add_aff(acc, a);
+        const uint4 *q = bases + 2 * C::FIELD_U4 * (uint64_t)(e & 0x7fffffffu);
+        typename C::Affine a; msm_ld(q, a.x); msm_ld(q + C::FIELD_U4, a.y);
+        if (e >> 31) a = pt_aff_neg(a);
+        acc = pt_add_aff(acc, a);
     }
 };
 // the entries of a later level: (key, partial sum) pairs, keys ascending, MSM_NONE last
-struct MsmPartials {
+template <class C> struct MsmPartials {
+    typedef C Curve;
     const uint32_t *keys;
-    const G1Xyzz *pts;
+    const typename C::Point *pts;
     uint32_t m;
     __device__ uint32_t count() const { return m; }
     __device__ uint32_t first_key(uint32_t p) const { return keys[p]; }
     __device__ uint32_t next_key(uint32_t, uint32_t p) const { return keys[p]; }
-    __device__ void add(G1Xyzz &acc, uint32_t p) const { acc = g1_add(acc, msm_ld_xyzz(pts + p)); }
+    __device__ void add(typename C::Point &acc, uint32_t p) const { acc = pt_add(acc, msm_ld_xyzz(pts + p)); }
 };
 
 // one level of the segmented reduction: T threads, thread t takes entries [t L, (t + 1) L), L = ceil(count / T).  A segment
@@ -190,86 +212,96 @@ struct MsmPartials {
 // 2t, the last to pair 2t + 1 (pair 2t + 1 is (key, O) when the chunk has one segment, both are (MSM_NONE, O) when it is empty).
 // With pkey == nullptr (the last level, T = 1) every segment is written to out.  Keys >= nb are not written.
 template <class Src>
-__global__ void __launch_bounds__(MSM_THREADS) k_msm_sum(Src src, uint32_t T, uint32_t nb, G1Xyzz *out, uint32_t *pkey, G1Xyzz *ppt) {
+__global__ void __launch_bounds__(MSM_THREADS) k_msm_sum(Src src, uint32_t T, uint32_t nb, typename Src::Curve::Point *out, uint32_t *pkey,
+                                                        typename Src::Curve::Point *ppt) {
+    typedef typename Src::Curve::Field F;
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= T) return;
     const uint32_t m = src.count(), L = (uint32_t)(((uint64_t)m + T - 1) / T);
     const uint32_t start = (uint32_t)min((uint64_t)t * L, (uint64_t)m), end = (uint32_t)min((uint64_t)start + L, (uint64_t)m);
     if (start >= end) {
-        if (pkey) { pkey[2 * t] = pkey[2 * t + 1] = MSM_NONE; msm_st_xyzz(ppt + 2 * t, g1_inf()); msm_st_xyzz(ppt + 2 * t + 1, g1_inf()); }
+        if (pkey) { pkey[2 * t] = pkey[2 * t + 1] = MSM_NONE; msm_st_xyzz(ppt + 2 * t, pt_inf<F>()); msm_st_xyzz(ppt + 2 * t + 1, pt_inf<F>()); }
         return;
     }
     uint32_t b = src.first_key(start);
     bool first = true;
-    G1Xyzz acc = g1_inf();
+    Xyzz<F> acc = pt_inf<F>();
     for (uint32_t p = start; p < end; p++) {
         const uint32_t k = src.next_key(b, p);
         if (k != b) {
             if (first && pkey) { pkey[2 * t] = b; msm_st_xyzz(ppt + 2 * t, acc); }
             else if (b < nb) msm_st_xyzz(out + b, acc);
-            first = false; b = k; acc = g1_inf();
+            first = false; b = k; acc = pt_inf<F>();
         }
         src.add(acc, p);
     }
     if (!pkey) { if (b < nb) msm_st_xyzz(out + b, acc); return; }
-    if (first) { pkey[2 * t] = b; msm_st_xyzz(ppt + 2 * t, acc); acc = g1_inf(); }
+    if (first) { pkey[2 * t] = b; msm_st_xyzz(ppt + 2 * t, acc); acc = pt_inf<F>(); }
     pkey[2 * t + 1] = b; msm_st_xyzz(ppt + 2 * t + 1, acc);
 }
 
 // thread g: sum_{b in [lo, lo + S)} (b + 1) B_b = sum (b - lo + 1) B_b (running sums from the top) + lo * sum B_b, as pair (0, .)
-__global__ void __launch_bounds__(MSM_THREADS) k_msm_reduce(const G1Xyzz *bkt, uint32_t K, uint32_t G, uint32_t *pkey, G1Xyzz *ppt) {
+template <class C>
+__global__ void __launch_bounds__(MSM_THREADS) k_msm_reduce(const typename C::Point *bkt, uint32_t K, uint32_t G, uint32_t *pkey, typename C::Point *ppt) {
+    typedef typename C::Field F;
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= G) return;
     const uint32_t lo = g * MSM_SEG, hi = min(lo + MSM_SEG, K);
-    G1Xyzz run = g1_inf(), acc = g1_inf();
-    for (uint32_t b = hi; b-- > lo;) { run = g1_add(run, msm_ld_xyzz(bkt + b)); acc = g1_add(acc, run); }
+    Xyzz<F> run = pt_inf<F>(), acc = pt_inf<F>();
+    for (uint32_t b = hi; b-- > lo;) { run = pt_add(run, msm_ld_xyzz(bkt + b)); acc = pt_add(acc, run); }
     pkey[g] = 0;
-    msm_st_xyzz(ppt + g, g1_add(acc, g1_mul_u32(run, lo)));
+    msm_st_xyzz(ppt + g, pt_add(acc, pt_mul_u32(run, lo)));
 }
 
-// sum_j 2^(c j) W_j, then canonical affine x, y into out (64 bytes)
-__global__ void k_msm_final(const G1Xyzz *win, uint32_t W, uint32_t c, uint4 *out) {
-    G1Xyzz acc = g1_inf();
+// sum_j 2^(c j) W_j, then canonical affine x, y into out (C::AFF_BYTES: 64 bytes for G1, 128 for G2)
+template <class C>
+__global__ void k_msm_final(const typename C::Point *win, uint32_t W, uint32_t c, uint4 *out) {
+    typedef typename C::Field F;
+    Xyzz<F> acc = pt_inf<F>();
     for (uint32_t j = W; j-- > 0;) {
-        if (!g1_is_inf(acc)) for (uint32_t k = 0; k < c; k++) acc = g1_dbl(acc);
-        acc = g1_add(acc, msm_ld_xyzz(win + j));
+        if (!pt_is_inf(acc)) for (uint32_t k = 0; k < c; k++) acc = pt_dbl(acc);
+        acc = pt_add(acc, msm_ld_xyzz(win + j));
     }
-    const G1Aff a = g1_to_affine_canonical(acc);
-    msm_st_fq(out, a.x); msm_st_fq(out + 2, a.y);
+    const Aff<F> a = pt_to_affine_canonical(acc);
+    msm_st(out, a.x); msm_st(out + C::FIELD_U4, a.y);
 }
 
 // reduce m (key, sum) pairs at (ka, pa) into out[key < nb], ping-ponging with (kb, pb)
-static void msm_cascade(uint32_t m, uint32_t nb, G1Xyzz *out, uint32_t *ka, G1Xyzz *pa, uint32_t *kb, G1Xyzz *pb, cudaStream_t st) {
+template <class C>
+static void msm_cascade(uint32_t m, uint32_t nb, typename C::Point *out, uint32_t *ka, typename C::Point *pa, uint32_t *kb, typename C::Point *pb,
+                        cudaStream_t st) {
     while (m > MSM_FINAL) {
         const uint32_t T = (m + MSM_PAIRS - 1) / MSM_PAIRS;
-        k_msm_sum<MsmPartials><<<(T + MSM_THREADS - 1) / MSM_THREADS, MSM_THREADS, 0, st>>>(MsmPartials{ka, pa, m}, T, nb, out, kb, pb);
+        k_msm_sum<MsmPartials<C>><<<(T + MSM_THREADS - 1) / MSM_THREADS, MSM_THREADS, 0, st>>>(MsmPartials<C>{ka, pa, m}, T, nb, out, kb, pb);
         std::swap(ka, kb); std::swap(pa, pb);
         m = 2 * T;
     }
-    k_msm_sum<MsmPartials><<<1, 1, 0, st>>>(MsmPartials{ka, pa, m}, 1, nb, out, nullptr, nullptr);
+    k_msm_sum<MsmPartials<C>><<<1, 1, 0, st>>>(MsmPartials<C>{ka, pa, m}, 1, nb, out, nullptr, nullptr);
 }
 
-// enqueue the whole multi-exponentiation on st; work holds msm_layout(n).bytes
-static cudaError_t msm_g1_enqueue(const uint4 *bases, const uint4 *scalars, uint64_t n, uint4 *out, uint8_t *work, uint32_t n_sms, cudaStream_t st) {
-    const MsmLayout L = msm_layout(n);
+// enqueue the whole multi-exponentiation on st; work holds msm_layout<C>(n).bytes, out C::AFF_BYTES
+template <class C>
+static cudaError_t msm_enqueue(const uint4 *bases, const uint4 *scalars, uint64_t n, uint4 *out, uint8_t *work, uint32_t n_sms, cudaStream_t st) {
+    typedef typename C::Point Pt;
+    const MsmLayout L = msm_layout<C>(n);
     uint32_t *idx = (uint32_t *)(work + L.idx), *cnt = (uint32_t *)(work + L.cnt), *offs = (uint32_t *)(work + L.offs);
     uint32_t *ka = (uint32_t *)(work + L.keys_a), *kb = (uint32_t *)(work + L.keys_b);
-    G1Xyzz *bkt = (G1Xyzz *)(work + L.bkt), *pa = (G1Xyzz *)(work + L.pts_a), *pb = (G1Xyzz *)(work + L.pts_b), *win = (G1Xyzz *)(work + L.win);
+    Pt *bkt = (Pt *)(work + L.bkt), *pa = (Pt *)(work + L.pts_a), *pb = (Pt *)(work + L.pts_b), *win = (Pt *)(work + L.win);
     const unsigned dgrid = (unsigned)std::min<uint64_t>((n + 255) / 256, 16ull * n_sms);
     const unsigned sgrid = (L.chunks + MSM_THREADS - 1) / MSM_THREADS;
     for (uint32_t j = 0; j < L.windows; j++) {
         cudaError_t e = cudaMemsetAsync(cnt, 0, 4ull * (L.buckets + 1), st);
-        if (e == cudaSuccess) e = cudaMemsetAsync(bkt, 0, sizeof(G1Xyzz) * (uint64_t)L.buckets, st);     // O everywhere
+        if (e == cudaSuccess) e = cudaMemsetAsync(bkt, 0, sizeof(Pt) * (uint64_t)L.buckets, st);     // O everywhere
         if (e != cudaSuccess) return e;
         k_msm_digits<false><<<dgrid, 256, 0, st>>>(scalars, n, L.c, j, cnt, nullptr);
         k_msm_scan<<<1, 1024, 0, st>>>(cnt, L.buckets, offs);
         k_msm_digits<true><<<dgrid, 256, 0, st>>>(scalars, n, L.c, j, cnt, idx);
-        k_msm_sum<MsmBases><<<sgrid, MSM_THREADS, 0, st>>>(MsmBases{offs, idx, bases, L.buckets}, L.chunks, L.buckets, bkt, ka, pa);
-        msm_cascade(2 * L.chunks, L.buckets, bkt, ka, pa, kb, pb, st);
-        k_msm_reduce<<<(L.seg_threads + MSM_THREADS - 1) / MSM_THREADS, MSM_THREADS, 0, st>>>(bkt, L.buckets, L.seg_threads, ka, pa);
-        msm_cascade(L.seg_threads, 1, win + j, ka, pa, kb, pb, st);
+        k_msm_sum<MsmBases<C>><<<sgrid, MSM_THREADS, 0, st>>>(MsmBases<C>{offs, idx, bases, L.buckets}, L.chunks, L.buckets, bkt, ka, pa);
+        msm_cascade<C>(2 * L.chunks, L.buckets, bkt, ka, pa, kb, pb, st);
+        k_msm_reduce<C><<<(L.seg_threads + MSM_THREADS - 1) / MSM_THREADS, MSM_THREADS, 0, st>>>(bkt, L.buckets, L.seg_threads, ka, pa);
+        msm_cascade<C>(L.seg_threads, 1, win + j, ka, pa, kb, pb, st);
     }
-    k_msm_final<<<1, 1, 0, st>>>(win, L.windows, L.c, out);
+    k_msm_final<C><<<1, 1, 0, st>>>(win, L.windows, L.c, out);
     return cudaGetLastError();
 }
 

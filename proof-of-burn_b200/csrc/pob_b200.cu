@@ -27,7 +27,7 @@
 #include "../../include/pob_b200.h"
 #include "compiler.h"
 #include "kernels.cuh"
-#include "msm.cuh"
+#include "groth16.cuh"
 #include "ntt.cuh"
 #include "r1cs.h"
 
@@ -1100,6 +1100,29 @@ static const NttTables &ensure_ntt(pob_handle *h, uint32_t L) {
     return N.t;
 }
 
+// q of witness slot s into out (n x 32 B), with work (2 n x 32 B) as scratch, enqueued on st
+static void quotient_enqueue(pob_handle *h, pob_handle::DevCons &C, const NttTables &T, uint32_t L, const uint64_t *s, uint4 *out, uint4 *work,
+                             cudaStream_t st) {
+    const uint64_t n = 1ull << L, m = C.info.n_constraints, np1 = h->P.n_outputs + 1;
+    uint4 *va = out, *vb = work, *vc = vb + 2 * n;                           // 2 uint4 per entry
+    // rows: [0, m) the products, m + s (s <= n_pub) a = w[s], the rest 0
+    if (m) {
+        R1csArgs ra{C.flat, C.round, C.konst, s, C.bases, 0, m, va, vb, vc};
+        k_r1cs_products<<<(unsigned)std::min<uint64_t>((2 * m + 255) / 256, h->n_sms * 16ull), 256, 0, st>>>(ra);
+        CU(cudaGetLastError());
+    }
+    CU(cudaMemcpyAsync(va + 2 * m, s, np1 * 32, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemsetAsync(va + 2 * (m + np1), 0, (n - m - np1) * 32, st));
+    CU(cudaMemsetAsync(vb + 2 * m, 0, (n - m) * 32, st));
+    CU(cudaMemsetAsync(vc + 2 * m, 0, (n - m) * 32, st));
+    const uint32_t tl = std::min(L, NTT_TILE_LOG);
+    for (uint4 *x : {va, vb, vc}) {                                          // coefficients on the coset, then their values there
+        CU(ntt_inverse_coset(x, L, tl, T, st));
+        if (x == vc) CU(ntt_forward(x, L, tl, T, st, va, vb, va));           // q = A.B - C, over A in out
+        else CU(ntt_forward(x, L, tl, T, st));
+    }
+}
+
 int pob_r1cs_domain(pob_handle *h, uint32_t *log_n) {
     if (!h || !log_n) return fail(POB_E_BAD_ARG, "pob_r1cs_domain: null argument");
     try {
@@ -1119,63 +1142,129 @@ int pob_r1cs_quotient(pob_handle *h, uint32_t index, void *out, void *work, void
         uint32_t L = 0;
         if (!r1cs_log_n(h, &L)) return fail(POB_E_RANGE, "pob_r1cs_quotient: the domain exceeds 2^28 points");
         const NttTables &T = ensure_ntt(h, L);
-        const uint64_t n = 1ull << L, m = C.info.n_constraints, np1 = h->P.n_outputs + 1;
+        const uint64_t n = 1ull << L;
         const uintptr_t o = (uintptr_t)out, w = (uintptr_t)work;
         if (o < w + 64 * n && w < o + 32 * n) return fail(POB_E_BAD_ARG, "pob_r1cs_quotient: work overlaps out");
         const cudaStream_t st = (cudaStream_t)consumer_stream;
-        uint4 *va = (uint4 *)out, *vb = (uint4 *)work, *vc = vb + 2 * n;        // 2 uint4 per entry
-        // rows: [0, m) the products, m + s (s <= n_pub) a = w[s], the rest 0
-        if (m) {
-            R1csArgs ra{C.flat, C.round, C.konst, s, C.bases, 0, m, va, vb, vc};
-            k_r1cs_products<<<(unsigned)std::min<uint64_t>((2 * m + 255) / 256, h->n_sms * 16ull), 256, 0, st>>>(ra);
-            CU(cudaGetLastError());
-        }
-        CU(cudaMemcpyAsync(va + 2 * m, s, np1 * 32, cudaMemcpyDeviceToDevice, st));
-        CU(cudaMemsetAsync(va + 2 * (m + np1), 0, (n - m - np1) * 32, st));
-        CU(cudaMemsetAsync(vb + 2 * m, 0, (n - m) * 32, st));
-        CU(cudaMemsetAsync(vc + 2 * m, 0, (n - m) * 32, st));
-        const uint32_t tl = std::min(L, NTT_TILE_LOG);
-        for (uint4 *x : {va, vb, vc}) {                                          // coefficients on the coset, then their values there
-            CU(ntt_inverse_coset(x, L, tl, T, st));
-            if (x == vc) CU(ntt_forward(x, L, tl, T, st, va, vb, va));           // q = A.B - C, over A in out
-            else CU(ntt_forward(x, L, tl, T, st));
-        }
+        quotient_enqueue(h, C, T, L, s, (uint4 *)out, (uint4 *)work, st);
         if (!consumer_stream) CU(cudaStreamSynchronize(st));
     } catch (const std::exception &e) { return fail(POB_E_CUDA, std::string("pob_r1cs_quotient: ") + e.what()); }
     return POB_OK;
 }
 
-// ---- the G1 multi-exponentiation (msm.cuh) -----------------------------------------------------------------------------
-int pob_msm_g1_work_bytes(uint64_t n, uint64_t *bytes) {
-    if (!bytes || n == 0) return fail(POB_E_BAD_ARG, "pob_msm_g1_work_bytes: null argument or n == 0");
-    if (n > MSM_MAX_N) return fail(POB_E_RANGE, "pob_msm_g1_work_bytes: n exceeds 2^31");
-    *bytes = msm_layout(n).bytes;
+// ---- the G1 and G2 multi-exponentiations (msm.cuh) ---------------------------------------------------------------------
+}  // extern "C"
+
+static bool overlap(const void *a, uint64_t na, const void *b, uint64_t nb) {
+    const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
+    return x < y + nb && y < x + na;
+}
+
+template <class C> static int msm_work_bytes(const char *who, uint64_t n, uint64_t *bytes) {
+    if (!bytes || n == 0) return fail(POB_E_BAD_ARG, std::string(who) + ": null argument or n == 0");
+    if (n > MSM_MAX_N) return fail(POB_E_RANGE, std::string(who) + ": n exceeds 2^31");
+    *bytes = msm_layout<C>(n).bytes;
     return POB_OK;
 }
 
-int pob_msm_g1(int device, const void *bases, const void *scalars, uint64_t n, void *out, void *work, uint64_t work_bytes, void *consumer_stream) {
-    if (!bases || !scalars || !out || !work || n == 0) return fail(POB_E_BAD_ARG, "pob_msm_g1: null argument or n == 0");
-    if (misaligned16({bases, scalars, out, work})) return fail(POB_E_BAD_ARG, "pob_msm_g1: bases, scalars, out and work must be 16-byte aligned");
-    if (n > MSM_MAX_N) return fail(POB_E_RANGE, "pob_msm_g1: n exceeds 2^31");
-    const uint64_t need = msm_layout(n).bytes;
-    if (work_bytes < need) return fail(POB_E_BAD_ARG, "pob_msm_g1: work is shorter than pob_msm_g1_work_bytes(n) = " + std::to_string(need));
-    auto overlap = [](const void *a, uint64_t na, const void *b, uint64_t nb) {
-        const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
-        return x < y + nb && y < x + na;
-    };
-    if (overlap(work, need, bases, 64 * n) || overlap(work, need, scalars, 32 * n) || overlap(work, need, out, 64))
-        return fail(POB_E_BAD_ARG, "pob_msm_g1: work overlaps bases, scalars or out");
-    if (overlap(out, 64, bases, 64 * n) || overlap(out, 64, scalars, 32 * n)) return fail(POB_E_BAD_ARG, "pob_msm_g1: out overlaps bases or scalars");
+template <class C>
+static int msm_call(const char *who, int device, const void *bases, const void *scalars, uint64_t n, void *out, void *work, uint64_t work_bytes,
+                    void *consumer_stream) {
+    const std::string w(who);
+    const uint64_t pb = C::AFF_BYTES;
+    if (!bases || !scalars || !out || !work || n == 0) return fail(POB_E_BAD_ARG, w + ": null argument or n == 0");
+    if (misaligned16({bases, scalars, out, work})) return fail(POB_E_BAD_ARG, w + ": bases, scalars, out and work must be 16-byte aligned");
+    if (n > MSM_MAX_N) return fail(POB_E_RANGE, w + ": n exceeds 2^31");
+    const uint64_t need = msm_layout<C>(n).bytes;
+    if (work_bytes < need) return fail(POB_E_BAD_ARG, w + ": work is shorter than " + w + "_work_bytes(n) = " + std::to_string(need));
+    if (overlap(work, need, bases, pb * n) || overlap(work, need, scalars, 32 * n) || overlap(work, need, out, pb))
+        return fail(POB_E_BAD_ARG, w + ": work overlaps bases, scalars or out");
+    if (overlap(out, pb, bases, pb * n) || overlap(out, pb, scalars, 32 * n)) return fail(POB_E_BAD_ARG, w + ": out overlaps bases or scalars");
     int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) return fail(POB_E_NO_DEVICE, "pob_msm_g1: no such CUDA device");
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) return fail(POB_E_NO_DEVICE, w + ": no such CUDA device");
     try {
         CU(cudaSetDevice(device));
         int sms = 0;
         CU(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
         const cudaStream_t st = (cudaStream_t)consumer_stream;
-        CU(msm_g1_enqueue((const uint4 *)bases, (const uint4 *)scalars, n, (uint4 *)out, (uint8_t *)work, (uint32_t)sms, st));
+        CU(msm_enqueue<C>((const uint4 *)bases, (const uint4 *)scalars, n, (uint4 *)out, (uint8_t *)work, (uint32_t)sms, st));
         if (!consumer_stream) CU(cudaStreamSynchronize(st));
-    } catch (const std::exception &e) { return fail(POB_E_CUDA, std::string("pob_msm_g1: ") + e.what()); }
+    } catch (const std::exception &e) { return fail(POB_E_CUDA, w + ": " + e.what()); }
+    return POB_OK;
+}
+
+extern "C" {
+
+int pob_msm_g1_work_bytes(uint64_t n, uint64_t *bytes) { return msm_work_bytes<MsmG1>("pob_msm_g1_work_bytes", n, bytes); }
+int pob_msm_g1(int device, const void *bases, const void *scalars, uint64_t n, void *out, void *work, uint64_t work_bytes, void *consumer_stream) {
+    return msm_call<MsmG1>("pob_msm_g1", device, bases, scalars, n, out, work, work_bytes, consumer_stream);
+}
+int pob_msm_g2_work_bytes(uint64_t n, uint64_t *bytes) { return msm_work_bytes<MsmG2>("pob_msm_g2_work_bytes", n, bytes); }
+int pob_msm_g2(int device, const void *bases, const void *scalars, uint64_t n, void *out, void *work, uint64_t work_bytes, void *consumer_stream) {
+    return msm_call<MsmG2>("pob_msm_g2", device, bases, scalars, n, out, work, work_bytes, consumer_stream);
+}
+
+// ---- the proof (groth16.cuh) -----------------------------------------------------------------------------------------------
+static int groth16_shape(pob_handle *h, const char *who, uint32_t *log_n) {
+    try {
+        CU(cudaSetDevice(h->device));
+        if (!r1cs_log_n(h, log_n)) return fail(POB_E_RANGE, std::string(who) + ": the domain exceeds 2^28 points");
+    } catch (const std::exception &e) { return fail(POB_E_CUDA, std::string(who) + ": " + e.what()); }
+    if (h->P.n_signals > MSM_MAX_N) return fail(POB_E_RANGE, std::string(who) + ": the witness exceeds 2^31 entries");
+    return POB_OK;
+}
+
+int pob_groth16_work_bytes(pob_handle *h, uint64_t *bytes) {
+    if (!h || !bytes) return fail(POB_E_BAD_ARG, "pob_groth16_work_bytes: null argument");
+    uint32_t L = 0;
+    if (int rc = groth16_shape(h, "pob_groth16_work_bytes", &L)) return rc;
+    *bytes = groth16_layout(1ull << L, h->P.n_signals, h->P.n_outputs).bytes;
+    return POB_OK;
+}
+
+int pob_groth16_prove(pob_handle *h, uint32_t index, const pob_groth16_key *key, const uint64_t r[4], const uint64_t s[4], void *proof, void *work,
+                      uint64_t work_bytes, void *consumer_stream) {
+    const char *who = "pob_groth16_prove";
+    if (!h || !key || !r || !s || !proof || !work) return fail(POB_E_BAD_ARG, "pob_groth16_prove: null argument");
+    uint32_t L = 0;
+    if (int rc = groth16_shape(h, who, &L)) return rc;
+    const uint64_t n = 1ull << L, nv = h->P.n_signals, np = h->P.n_outputs, nc = nv - np - 1;
+    if (key->n_vars != nv || key->n_pub != np || key->log_n != L)
+        return fail(POB_E_BAD_ARG, "pob_groth16_prove: the key's n_vars, n_pub or log_n differs from the handle's (" + std::to_string(nv) + ", " +
+                    std::to_string(np) + ", " + std::to_string(L) + ")");
+    const void *pts[] = {key->alpha1, key->beta1, key->delta1, key->beta2, key->delta2, key->a, key->b1, key->b2, key->c, key->h};
+    for (const void *p : pts) if (!p) return fail(POB_E_BAD_ARG, "pob_groth16_prove: null key pointer");
+    if (misaligned16({key->alpha1, key->beta1, key->delta1, key->beta2, key->delta2, key->a, key->b1, key->b2, key->c, key->h, proof, work}))
+        return fail(POB_E_BAD_ARG, "pob_groth16_prove: key points, proof and work must be 16-byte aligned");
+    const Groth16Layout G = groth16_layout(n, nv, np);
+    if (work_bytes < G.bytes) return fail(POB_E_BAD_ARG, "pob_groth16_prove: work is shorter than pob_groth16_work_bytes = " + std::to_string(G.bytes));
+    if (overlap(proof, 256, work, G.bytes)) return fail(POB_E_BAD_ARG, "pob_groth16_prove: proof overlaps work");
+    uint64_t *w = nullptr; int rc = resident_slot(h, index, &w, (cudaStream_t)consumer_stream); if (rc) return rc;
+    try {
+        pob_handle::DevCons &C = ensure_r1cs(h);
+        const NttTables &T = ensure_ntt(h, L);
+        const cudaStream_t st = (cudaStream_t)consumer_stream;
+        uint8_t *wk = (uint8_t *)work;
+        uint4 *q = (uint4 *)(wk + G.q), *out = (uint4 *)proof;
+        uint8_t *scratch = wk + G.scratch;
+        auto res = [&](uint64_t off) { return (uint4 *)(wk + off); };
+        quotient_enqueue(h, C, T, L, w, q, (uint4 *)scratch, st);
+        CU(msm_enqueue<MsmG1>((const uint4 *)key->h, q, n, res(G.h), scratch, h->n_sms, st));
+        CU(msm_enqueue<MsmG1>((const uint4 *)key->a, (const uint4 *)w, nv, res(G.a), scratch, h->n_sms, st));
+        CU(msm_enqueue<MsmG1>((const uint4 *)key->b1, (const uint4 *)w, nv, res(G.b1), scratch, h->n_sms, st));
+        if (nc) CU(msm_enqueue<MsmG1>((const uint4 *)key->c, (const uint4 *)(w + 4 * (np + 1)), nc, res(G.c), scratch, h->n_sms, st));
+        else CU(cudaMemsetAsync(res(G.c), 0, 64, st));                   // no private wire: the C sum is O
+        CU(msm_enqueue<MsmG2>((const uint4 *)key->b2, (const uint4 *)w, nv, res(G.b2), scratch, h->n_sms, st));
+        Groth16Assemble ga{(const uint4 *)key->alpha1, (const uint4 *)key->beta1, (const uint4 *)key->delta1, (const uint4 *)key->beta2,
+                           (const uint4 *)key->delta2, res(G.h), res(G.a), res(G.b1), res(G.c), res(G.b2), {}, {}, out};
+        for (int i = 0; i < 4; i++) {
+            ga.r[2 * i] = (uint32_t)r[i]; ga.r[2 * i + 1] = (uint32_t)(r[i] >> 32);
+            ga.s[2 * i] = (uint32_t)s[i]; ga.s[2 * i + 1] = (uint32_t)(s[i] >> 32);
+        }
+        k_groth16_assemble<<<1, 1, 0, st>>>(ga);
+        CU(cudaGetLastError());
+        if (!consumer_stream) CU(cudaStreamSynchronize(st));
+    } catch (const std::exception &e) { return fail(POB_E_CUDA, std::string("pob_groth16_prove: ") + e.what()); }
     return POB_OK;
 }
 

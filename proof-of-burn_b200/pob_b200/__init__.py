@@ -13,6 +13,7 @@ decimal strings, nested arrays, scalars possibly wrapped in 1-element arrays).
 All witness computation happens in hand-written CUDA (csrc/pob_b200.cu).  There is no CPU fallback: if the
 extension is missing or no GPU is visible, construction fails loudly.
 """
+import collections
 import ctypes
 import json
 import os
@@ -21,6 +22,7 @@ import re
 import numpy as np
 
 P = 21888242871839275222246405745257275088548364400416034343698204186575808495617
+R_ORDER = P                                       # BN254's group order r is the scalar field's modulus
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libpob_b200.so")
 
@@ -81,6 +83,40 @@ class R1csDesc(ctypes.Structure):
 
     def as_dict(self):
         return {k: int(getattr(self, k)) for k, _ in self._fields_}
+
+
+class Groth16KeyC(ctypes.Structure):
+    """pob_b200.h: pob_groth16_key"""
+    _fields_ = [("n_vars", ctypes.c_uint64), ("n_pub", ctypes.c_uint32), ("log_n", ctypes.c_uint32)] + \
+        [(f, ctypes.c_void_p) for f in ("alpha1", "beta1", "delta1", "beta2", "delta2", "a", "b1", "b2", "c", "h")]
+
+
+class Groth16Key(collections.namedtuple("Groth16Key", "alpha1 beta1 delta1 beta2 delta2 a b1 b2 c h")):
+    """A Groth16 proving key as CUDA tensors (pob_b200.h: pob_groth16_key): G1 points are (k, 8) uint64 tensors and G2 points (k, 16),
+    affine, Montgomery-form F_q limbs as msm_g1 / msm_g2 take them.  alpha1, beta1, delta1: one G1 point each; beta2, delta2: one G2
+    point each; a, b1: n_signals G1 points; b2: n_signals G2 points; c: n_signals - n_outputs - 1 G1 points (wires n_outputs + 1 ..);
+    h: 2^r1cs_domain() G1 points, paired with the quotient's q[k]."""
+
+
+class Proof(collections.namedtuple("Proof", "a b c")):
+    """A Groth16 proof as ints: a and c are G1 points (x, y), b a G2 point ((x0, x1), (y0, y1)) with x = x0 + x1 u; None = infinity."""
+
+    def to_json(self):
+        """the proof.json dictionary of snarkjs (pi_a, pi_b, pi_c as projective decimal strings with z = 1, pi_b coordinates as
+        [c0, c1]).  The shape follows snarkjs as far as it is known here; it has not been checked against snarkjs."""
+        def g1(p):
+            return ["0", "1", "0"] if p is None else [str(p[0]), str(p[1]), "1"]
+
+        def g2(p):
+            if p is None:
+                return [["0", "0"], ["1", "0"], ["0", "0"]]
+            return [[str(p[0][0]), str(p[0][1])], [str(p[1][0]), str(p[1][1])], ["1", "0"]]
+        return {"pi_a": g1(self.a), "pi_b": g2(self.b), "pi_c": g1(self.c), "protocol": "groth16", "curve": "bn128"}
+
+
+def public_json(outputs):
+    """the public signals of a proof (snarkjs public.json: decimal strings), from the circuit's outputs (BatchResult.outputs[i])"""
+    return [str(int(v) % P) for v in outputs]
 
 
 _LIB = None
@@ -155,6 +191,14 @@ def lib():
         L.pob_msm_g1_work_bytes.argtypes = [u64, ctypes.POINTER(u64)]
         L.pob_msm_g1.restype = ci
         L.pob_msm_g1.argtypes = [ci, vp, vp, u64, vp, vp, u64, vp]
+        L.pob_msm_g2_work_bytes.restype = ci
+        L.pob_msm_g2_work_bytes.argtypes = [u64, ctypes.POINTER(u64)]
+        L.pob_msm_g2.restype = ci
+        L.pob_msm_g2.argtypes = [ci, vp, vp, u64, vp, vp, u64, vp]
+        L.pob_groth16_work_bytes.restype = ci
+        L.pob_groth16_work_bytes.argtypes = [vp, ctypes.POINTER(u64)]
+        L.pob_groth16_prove.restype = ci
+        L.pob_groth16_prove.argtypes = [vp, u32, ctypes.POINTER(Groth16KeyC), vp, vp, vp, vp, u64, vp]
         L.pob_pow_grind.restype = ci
         L.pob_pow_grind.argtypes = [ci, vp, vp, vp, u32, u64, vp, ctypes.POINTER(u64)]
         L.pob_last_error.restype = ctypes.c_char_p
@@ -541,6 +585,42 @@ class Circuit:
         _check(lib().pob_r1cs_quotient(self._h, index, out.data_ptr(), work.data_ptr(), handle))
         return out
 
+    def groth16_work_bytes(self):
+        """bytes of scratch groth16_prove needs on this circuit (pob_groth16_work_bytes)"""
+        v = ctypes.c_uint64(0)
+        _check(lib().pob_groth16_work_bytes(self._h, ctypes.byref(v)))
+        return int(v.value)
+
+    def groth16_prove(self, index, key, r=None, s=None, stream=None, out=None, work=None):
+        """a Groth16 proof of resident witness `index` on the GPU (pob_b200.h: pob_groth16_prove) with a Groth16Key.  r and s are the
+        blinding scalars; each defaults to secrets.randbelow(R_ORDER), as zero knowledge needs.  Returns a Proof of ints; with a stream
+        (torch.cuda.Stream or raw cudaStream_t) the work and any out / work tensor it allocates are enqueued on it, and the (32,) uint64
+        out tensor (A: 8 limbs, B: 16, C: 8, canonical) is returned unsynchronised."""
+        import secrets
+        import torch
+        r = secrets.randbelow(R_ORDER) if r is None else int(r)
+        s = secrets.randbelow(R_ORDER) if s is None else int(s)
+        dev = torch.device("cuda", self.device)
+        handle = None if stream is None else getattr(stream, "cuda_stream", stream)
+        need = self.groth16_work_bytes()
+        with torch.cuda.stream(torch.cuda.ExternalStream(handle, device=dev) if handle else torch.cuda.current_stream(dev)):
+            if out is None:
+                out = torch.empty(32, dtype=torch.uint64, device=dev)
+            if work is None:
+                work = torch.empty(need, dtype=torch.uint8, device=dev)
+        for t, what in [(out, "out"), (work, "work")] + [(v, "key." + f) for f, v in zip(key._fields, key)]:
+            if not t.is_cuda or t.device != dev or not t.is_contiguous():
+                raise ValueError("groth16_prove: %s must be a contiguous tensor on %s" % (what, dev))
+        if out.numel() * out.element_size() < 256:
+            raise ValueError("groth16_prove: out must hold 256 bytes")
+        kc = Groth16KeyC(self.n_signals, self.n_outputs, self.r1cs_domain(), *[v.data_ptr() for v in key])
+        rl, sl = to_limbs([r % (1 << 256)]), to_limbs([s % (1 << 256)])
+        _check(lib().pob_groth16_prove(self._h, index, ctypes.byref(kc), rl.ctypes.data, sl.ctypes.data, out.data_ptr(), work.data_ptr(),
+                                       work.numel() * work.element_size(), handle))
+        if handle:
+            return out
+        return proof_from_limbs(out.cpu().tolist())
+
     def witness_map(self):
         m = np.zeros(self.n_signals, dtype=np.uint32)
         _check(lib().pob_witness_map(self._h, m.ctypes.data))
@@ -602,6 +682,56 @@ def msm_g1(bases, scalars, stream=None, out=None, work=None, device=None):
     v = [int(x) & ((1 << 64) - 1) for x in out.cpu().tolist()]
     x, y = (sum(v[4 * k + i] << (64 * i) for i in range(4)) for k in (0, 1))
     return None if x == 0 and y == 0 else (x, y)
+
+
+def _point(limbs, coords):
+    v = [int(x) & ((1 << 64) - 1) for x in limbs]
+    c = [sum(v[4 * k + i] << (64 * i) for i in range(4)) for k in range(coords)]
+    return c if any(c) else None
+
+
+def proof_from_limbs(limbs):
+    """Proof of ints from the 32 uint64 limbs pob_groth16_prove writes"""
+    a, b, c = _point(limbs[0:8], 2), _point(limbs[8:24], 4), _point(limbs[24:32], 2)
+    return Proof(None if a is None else tuple(a), None if b is None else ((b[0], b[1]), (b[2], b[3])), None if c is None else tuple(c))
+
+
+def msm_g2_work_bytes(n):
+    """bytes of scratch pob_msm_g2 needs for n points (host only, no GPU)"""
+    v = ctypes.c_uint64(0)
+    _check(lib().pob_msm_g2_work_bytes(int(n), ctypes.byref(v)))
+    return int(v.value)
+
+
+def msm_g2(bases, scalars, stream=None, out=None, work=None, device=None):
+    """sum_i [s_i] P_i over BN254 G2 on the GPU (pob_b200.h: pob_msm_g2).  bases: (n, 16) uint64 CUDA tensor, per point x.c0, x.c1,
+    y.c0, y.c1 as Montgomery-form F_q limbs, all-zero = infinity; points of the order-r subgroup (not checked).  scalars as msm_g1.
+    Returns ((x0, x1), (y0, y1)) as canonical ints, or None for infinity; with a stream the (16,) uint64 out tensor, unsynchronised."""
+    import torch
+    if isinstance(scalars, tuple):
+        s_ptr, n = int(scalars[0]), int(scalars[1])
+    else:
+        if scalars.dim() != 2 or scalars.shape[1] != 4 or scalars.dtype not in (torch.uint64, torch.int64) or not scalars.is_contiguous():
+            raise ValueError("msm_g2: scalars must be a contiguous (n, 4) uint64 tensor")
+        s_ptr, n = scalars.data_ptr(), scalars.shape[0]
+    if bases.dim() != 2 or bases.shape[1] != 16 or bases.shape[0] != n or bases.dtype not in (torch.uint64, torch.int64) or not bases.is_contiguous():
+        raise ValueError("msm_g2: bases must be a contiguous (n, 16) uint64 tensor with n = %d" % n)
+    dev = bases.device if device is None else torch.device("cuda", device)
+    handle = None if stream is None else getattr(stream, "cuda_stream", stream)
+    with torch.cuda.stream(torch.cuda.ExternalStream(handle, device=dev) if handle else torch.cuda.current_stream(dev)):
+        if out is None:
+            out = torch.empty(16, dtype=torch.uint64, device=dev)
+        if work is None:
+            work = torch.empty(msm_g2_work_bytes(n), dtype=torch.uint8, device=dev)
+    for t, what in ((bases, "bases"), (out, "out"), (work, "work")):
+        if not t.is_cuda or t.device != dev or not t.is_contiguous():
+            raise ValueError("msm_g2: %s must be a contiguous tensor on %s" % (what, dev))
+    _check(lib().pob_msm_g2(dev.index, bases.data_ptr(), s_ptr, n, out.data_ptr(), work.data_ptr(),
+                            work.numel() * work.element_size(), handle))
+    if handle:
+        return out
+    c = _point(out.cpu().tolist(), 4)
+    return None if c is None else ((c[0], c[1]), (c[2], c[3]))
 
 
 def repad_pob_input(inp, max_layers, node_blocks, header_blocks):
