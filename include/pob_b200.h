@@ -38,6 +38,7 @@ enum {
     POB_E_COMPILE = -7,       /* the layout compiler rejected the circuit shape */
     POB_E_REJECTED = -8,      /* the instance failed a circuit constraint: it has no witness (reference tests/test.py:65-68) */
     POB_E_BUSY = -9,          /* every witness slot is held by the consumer: release one first / a batch is in flight */
+    POB_E_KEY = -10,          /* a .zkey is malformed, does not fit the circuit, or fails its check (pob_zkey_info / pob_zkey_load) */
     POB_DONE = 1              /* pob_acquire: no further witness in this batch (not an error) */
 };
 
@@ -332,6 +333,64 @@ int pob_groth16_work_bytes(pob_handle *h, uint64_t *bytes);
 int pob_groth16_prove(pob_handle *h, uint32_t index, const pob_groth16_key *key,
                       const uint64_t r[4], const uint64_t s[4],
                       void *proof, void *work, uint64_t work_bytes, void *consumer_stream);
+
+/* ---- the proving key from a snarkjs .zkey ----------------------------------------------------------------------------------------
+ * The format as far as known here (not checked against a file written by snarkjs; DESIGN.md §5 "Key loading").  Integers are little
+ * endian.  "zkey", u32 version (1), u32 n_sections, then per section u32 id, u64 size, size bytes, in any order.  Ids 1..9 appear
+ * exactly once each; id 10 (contributions) and unknown ids are skipped.
+ *   1: u32 protocol (1 = Groth16)
+ *   2: u32 n8q (32), q, u32 n8r (32), r, u32 nVars, u32 nPublic, u32 domainSize, alpha1 G1, beta1 G1, beta2 G2, gamma2 G2, delta1 G1,
+ *      delta2 G2 (660 bytes)
+ *   3: nPublic + 1 G1 points (IC: checked, not returned)
+ *   4: u32 nCoefs, then nCoefs x 44 B: u32 matrix (0 = A, 1 = B), u32 constraint, u32 signal, value = c R^2 mod r (R = 2^256).
+ *      snarkjs appends the A entries (m + s, s, 1) for s = 0 .. nPublic: the public rows of pob_r1cs_quotient.  No C matrix.
+ *   5: A, nVars G1   6: B1, nVars G1   7: B2, nVars G2   8: C, nVars - nPublic - 1 G1   9: H, domainSize G1
+ * Points are affine, 64 B (G1) or 128 B (G2), Montgomery form, (0, 0) = infinity: the form of pob_msm_g1 / pob_msm_g2, so sections 5-9
+ * land in device memory byte for byte. */
+typedef struct {
+    uint64_t n_vars;           /* nVars   (== pob_desc.n_signals of a handle the key fits) */
+    uint32_t n_pub;            /* nPublic (== n_outputs) */
+    uint32_t log_n;            /* log2 domainSize (== pob_r1cs_domain) */
+    uint64_t n_coefs;          /* section-4 entries, the public rows included */
+    uint64_t file_bytes;
+    uint64_t a_bytes, b1_bytes, b2_bytes, c_bytes, h_bytes;   /* device bytes of pob_groth16_key.a, .b1, .b2, .c, .h */
+    uint64_t key_bytes;        /* those five plus alpha1, beta1, delta1 (64 B each) and beta2, delta2 (128 B each) */
+} pob_zkey_desc;
+/* host-only, no GPU needed: parse the header and the section table and validate the structure (magic, version, protocol, n8q / n8r,
+ * both moduli, one each of sections 1-9, every section size against nVars, nPublic, domainSize and nCoefs, domainSize a power of two
+ * <= 2^28).  A file that cannot be read or ends early: POB_E_IO; any structural error: POB_E_KEY; pob_last_error names it. */
+int pob_zkey_info(const char *path, pob_zkey_desc *out);
+
+typedef struct {
+    uint32_t coef_match;            /* bit 0: matrix A of section 4 equals the handle's .r1cs A rows plus the public rows, bit 1: B equals
+                                       B; values read as c R^2 mod r */
+    uint32_t coef_match_canonical;  /* the same bits with the values read as canonical elements (diagnosis of the encoding) */
+    uint64_t coef_out_of_range;     /* entries with matrix > 1, constraint >= domainSize or signal >= nVars (counted, never used) */
+    uint64_t points_checked;        /* points of sections 2, 3 and 5-9 */
+    uint64_t points_bad;            /* a coordinate >= q, or off the curve read in Montgomery form */
+    uint64_t points_bad_canonical;  /* the same with the coordinates read as canonical elements */
+    uint32_t first_bad_section;     /* section of the first bad point (smallest section, then index); 0 = none */
+    uint32_t reserved;
+    uint64_t first_bad_index;       /* its index in the section (section 2: 0 alpha1, 1 beta1, 2 beta2, 3 gamma2, 4 delta1, 5 delta2) */
+    float read_ms;                  /* host time in file reads (reader thread) */
+    float copy_ms;                  /* device time of the host-to-device copies */
+    float check_ms;                 /* device time of the check kernels (both sides of the coefficient check, the point checks) */
+    float total_ms;                 /* wall time of the call */
+    uint64_t bytes_read;
+    uint64_t device_scratch_bytes;  /* peak device memory the call allocated itself (freed before it returns) */
+} pob_zkey_report;
+/* Fill the caller's key buffers from a .zkey and check the key against the handle's circuit on the GPU.  dst: a pob_groth16_key whose
+ * n_vars / n_pub / log_n are the handle's and whose pointers are device buffers of the sizes pob_zkey_info gives (16-byte aligned);
+ * after success it is ready for pob_groth16_prove.  A key whose nVars, nPublic or domainSize differ from the handle's n_signals,
+ * n_outputs or pob_r1cs_domain is refused before any transfer (POB_E_KEY).  The file streams through a ring of pinned staging buffers
+ * of at most staging_bytes in all (0 = 256 MiB; at least 512), read by a host thread while earlier chunks are copied and checked; it is
+ * never held in host memory whole.  A setup call: it waits on the host, and allocates and frees device scratch (reported).
+ * The check: with pseudo-random x_j per wire and rho_c per domain row derived from `seed` on the device, for M = A, B
+ *   sum over section-4 entries (M, c, s, v) of rho_c x_s c   ==   sum_c rho_c (M x)_c   (k_r1cs_products over x, + the public rows for A),
+ * equal for equal matrices and, except with probability about 2 / r, different for any other; every point of sections 2, 3, 5-9 has
+ * coordinates < q and lies on y^2 = x^3 + 3 (G1) or the twist (G2) read in Montgomery form, or is (0, 0).  Not checked: the G2 subgroup.
+ * A failure of either part is POB_E_KEY with rep filled in (rep may be NULL). */
+int pob_zkey_load(pob_handle *h, const char *path, uint64_t seed, uint64_t staging_bytes, const pob_groth16_key *dst, pob_zkey_report *rep);
 
 /* ---- the step just before the path (SURVEY.md 8(f) rank 3) ------------------------------------------------------
  * replaces: find_burn_key() of the reference input generator (tests/main.py:47-56): starting at start_key, find the

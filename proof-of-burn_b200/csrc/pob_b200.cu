@@ -30,11 +30,14 @@
 #include "groth16.cuh"
 #include "ntt.cuh"
 #include "r1cs.h"
+#include "zkey.cuh"
+#include "zkey.h"
 
 using namespace pob;
 
 static thread_local std::string g_err;
 static int fail(int code, const std::string &msg) { g_err = msg; return code; }
+void pob_set_error(const std::string &msg) { g_err = msg; }   // for zkey.cpp
 #define CU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) throw std::runtime_error(std::string(#call) + ": " + cudaGetErrorString(e_)); } while (0)
 
 // Tuning / profiling knobs (POB_* environment variables) exist only in the -DPOB_TUNING build (`make tuning`, used by
@@ -1269,3 +1272,264 @@ int pob_groth16_prove(pob_handle *h, uint32_t index, const pob_groth16_key *key,
 }
 
 }  // extern "C"
+
+// ---- the proving key from a .zkey (zkey.h, zkey.cuh) ---------------------------------------------------------------------------
+// One host thread reads the file into a ring of pinned staging buffers, strictly round-robin; this thread issues each filled buffer:
+// point chunks are copied to their place in the caller's key (s_copy), coefficient chunks to a device buffer of the same ring slot,
+// where k_zkey_coefs consumes them (s_check).  Coefficient reads are cut at entry boundaries; point chunks need not be, since a
+// section's points are checked in the key itself once its last chunk has landed.  The row side of the coefficient check runs on
+// s_check first, while the reader fills the ring.
+namespace {
+
+struct ZkeyLoad {
+    static const int NB = 4;
+    int device = 0, fd = -1;
+    uint64_t S = 0;                                        // bytes per staging buffer
+    void *pin[NB] = {}; void *dcoef[NB] = {};
+    cudaStream_t s_copy = nullptr, s_check = nullptr;
+    cudaEvent_t c0[NB] = {}, c1[NB] = {}, k0[NB] = {}, k1[NB] = {};
+    bool c_rec[NB] = {}, k_rec[NB] = {};
+    std::vector<cudaEvent_t> ev;                           // start / end pairs of the other check kernels
+    std::vector<void *> dev; uint64_t dev_bytes = 0;
+    // reader
+    struct Job { uint32_t section; uint64_t off, bytes, dst_off; bool last; };
+    std::vector<Job> jobs;
+    std::mutex m; std::condition_variable cv; std::thread th;
+    std::vector<uint8_t> state;                            // per ring slot: 0 free / issued, 1 filled
+    size_t filled_upto = 0; bool stop = false, io_err = false; std::string cuda_err;
+    double read_ms = 0, copy_ms = 0;
+
+    void *alloc(uint64_t bytes) { void *p = nullptr; CU(cudaMalloc(&p, std::max<uint64_t>(bytes, 16))); dev.push_back(p); dev_bytes += std::max<uint64_t>(bytes, 16); return p; }
+    cudaEvent_t event() { cudaEvent_t e; CU(cudaEventCreate(&e)); ev.push_back(e); return e; }
+    ~ZkeyLoad() {
+        { std::lock_guard<std::mutex> l(m); stop = true; }
+        cv.notify_all();
+        if (th.joinable()) th.join();
+        if (s_copy) cudaStreamSynchronize(s_copy);
+        if (s_check) cudaStreamSynchronize(s_check);
+        for (void *p : dev) cudaFree(p);
+        for (int b = 0; b < NB; b++) {
+            if (pin[b]) cudaFreeHost(pin[b]);
+            for (cudaEvent_t e : {c0[b], c1[b], k0[b], k1[b]}) if (e) cudaEventDestroy(e);
+        }
+        for (cudaEvent_t e : ev) cudaEventDestroy(e);
+        for (cudaStream_t s : {s_copy, s_check}) if (s) cudaStreamDestroy(s);
+        if (fd >= 0) close(fd);
+    }
+    static float elapsed(cudaEvent_t a, cudaEvent_t b) { float ms = 0; CU(cudaEventElapsedTime(&ms, a, b)); return ms; }
+    void reader() {
+        cudaSetDevice(device);
+        for (size_t j = 0; j < jobs.size(); j++) {
+            const int b = (int)(j % NB);
+            {
+                std::unique_lock<std::mutex> l(m);
+                cv.wait(l, [&] { return stop || state[b] == 0; });
+                if (stop) return;
+            }
+            if (c_rec[b]) {                                // the slot's previous copy must be done before its buffer is overwritten
+                const cudaError_t e = cudaEventSynchronize(c1[b]);
+                if (e != cudaSuccess) { std::lock_guard<std::mutex> l(m); cuda_err = cudaGetErrorString(e); stop = true; cv.notify_all(); return; }
+                float ms = 0; cudaEventElapsedTime(&ms, c0[b], c1[b]); copy_ms += ms; c_rec[b] = false;
+            }
+            const auto t0 = std::chrono::steady_clock::now();
+            const bool ok = zkey_pread(fd, pin[b], jobs[j].bytes, jobs[j].off);
+            read_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+            std::lock_guard<std::mutex> l(m);
+            if (!ok) { io_err = true; stop = true; cv.notify_all(); return; }
+            state[b] = 1; filled_upto = j + 1;
+            cv.notify_all();
+        }
+    }
+};
+
+// the twist's b' = 3 / (9 + u) and G1's b = 3, in Montgomery form
+Fq zk_b1() { Fq t = fq_zero(); t.l[0] = 3; return fq_to_mont(t); }
+Fq2 zk_b2() {
+    Fq2 three = fq2_zero(), xi = fq2_zero();
+    three.c0.l[0] = 3; xi.c0.l[0] = 9; xi.c1.l[0] = 1;
+    return fq2_mul(fq2_to_mont(three), fq2_inv(fq2_to_mont(xi)));
+}
+
+}  // namespace
+
+extern "C" int pob_zkey_load(pob_handle *h, const char *path, uint64_t seed, uint64_t staging_bytes, const pob_groth16_key *dst, pob_zkey_report *rep) {
+    const char *who = "pob_zkey_load";
+    const auto t_start = std::chrono::steady_clock::now();
+    pob_zkey_report R{};
+    if (rep) *rep = R;
+    if (!h || !path || !dst) return fail(POB_E_BAD_ARG, "pob_zkey_load: null argument");
+    const uint64_t total_staging = staging_bytes ? staging_bytes : (256ull << 20);
+    if (total_staging < 512) return fail(POB_E_BAD_ARG, "pob_zkey_load: staging_bytes must be 0 or at least 512");
+    ZkeyLayout L;
+    try { L = zkey_parse(path); }
+    catch (const ZkeyError &e) { return fail(e.code, std::string(who) + ": " + path + ": " + e.what()); }
+    uint32_t log_n = 0;
+    if (int rc = groth16_shape(h, who, &log_n)) return rc;
+    const uint64_t nv = h->P.n_signals, np = h->P.n_outputs;
+    if (L.n_vars != nv) return fail(POB_E_KEY, std::string(who) + ": the key's nVars " + std::to_string(L.n_vars) + " differs from the circuit's n_signals " + std::to_string(nv));
+    if (L.n_pub != np) return fail(POB_E_KEY, std::string(who) + ": the key's nPublic " + std::to_string(L.n_pub) + " differs from the circuit's n_outputs " + std::to_string(np));
+    if (L.log_n != log_n) return fail(POB_E_KEY, std::string(who) + ": the key's domainSize 2^" + std::to_string(L.log_n) + " differs from the circuit's 2^" + std::to_string(log_n));
+    if (dst->n_vars != nv || dst->n_pub != np || dst->log_n != log_n) return fail(POB_E_BAD_ARG, "pob_zkey_load: dst's n_vars, n_pub or log_n differs from the handle's");
+    const void *pts[] = {dst->alpha1, dst->beta1, dst->delta1, dst->beta2, dst->delta2, dst->a, dst->b1, dst->b2, dst->c, dst->h};
+    for (const void *p : pts) if (!p) return fail(POB_E_BAD_ARG, "pob_zkey_load: null key pointer");
+    if (misaligned16({dst->alpha1, dst->beta1, dst->delta1, dst->beta2, dst->delta2, dst->a, dst->b1, dst->b2, dst->c, dst->h}))
+        return fail(POB_E_BAD_ARG, "pob_zkey_load: key pointers must be 16-byte aligned");
+    try {
+        CU(cudaSetDevice(h->device));
+        pob_handle::DevCons &C = ensure_r1cs(h);
+        const uint64_t m = C.info.n_constraints, domain = 1ull << log_n;
+        ZkeyLoad Z;
+        Z.device = h->device; Z.S = total_staging / ZkeyLoad::NB;
+        Z.fd = open(path, O_RDONLY);
+        if (Z.fd < 0) return fail(POB_E_IO, std::string(who) + ": cannot open " + path);
+        // the chunks of sections 4..9, in file order
+        uint8_t *const dsec[ZK_N_IDS] = {nullptr, nullptr, nullptr, nullptr, nullptr, (uint8_t *)dst->a, (uint8_t *)dst->b1, (uint8_t *)dst->b2, (uint8_t *)dst->c, (uint8_t *)dst->h};
+        std::vector<uint32_t> order;
+        for (uint32_t id = 4; id <= 9; id++) order.push_back(id);
+        std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return L.off[a] < L.off[b]; });
+        const uint64_t coef_chunk = Z.S / ZK_ENTRY_BYTES * ZK_ENTRY_BYTES;
+        for (uint32_t id : order) {
+            const uint64_t begin = id == 4 ? 4 : 0, size = L.size[id], step = id == 4 ? coef_chunk : Z.S;
+            for (uint64_t o = begin; o < size; o += step) {
+                const uint64_t b = std::min(step, size - o);
+                Z.jobs.push_back(ZkeyLoad::Job{id, L.off[id] + o, b, o, o + b == size});
+            }
+        }
+        Z.state.assign(ZkeyLoad::NB, 0);
+        CU(cudaStreamCreateWithFlags(&Z.s_copy, cudaStreamNonBlocking));
+        CU(cudaStreamCreateWithFlags(&Z.s_check, cudaStreamNonBlocking));
+        for (int b = 0; b < ZkeyLoad::NB; b++) {
+            CU(cudaMallocHost(&Z.pin[b], Z.S));
+            for (cudaEvent_t *e : {&Z.c0[b], &Z.c1[b], &Z.k0[b], &Z.k1[b]}) CU(cudaEventCreate(e));
+            if (L.n_coefs) Z.dcoef[b] = Z.alloc(std::min<uint64_t>(coef_chunk, L.size[4]));
+        }
+        // device scratch: x, two row windows, the block slots of both sides, the counters, the points of sections 2 and 3 (16-byte
+        // aligned: the point kernels load uint4)
+        const uint32_t slots = h->n_sms * 2;
+        const uint64_t W = std::max<uint64_t>(1, std::min<uint64_t>(m, 1ull << 20));
+        uint4 *x = (uint4 *)Z.alloc(32 * nv), *wa = (uint4 *)Z.alloc(32 * W), *wb = (uint4 *)Z.alloc(32 * W);
+        Fr *coef_acc = (Fr *)Z.alloc(64ull * slots), *row_acc = (Fr *)Z.alloc(64ull * slots);
+        ZkeyCounters *ctr = (ZkeyCounters *)Z.alloc(sizeof(ZkeyCounters));
+        const uint64_t sec2_pts = ZK_SEC2_BYTES - ZK_SEC2_POINTS;           // 576 = 36 x 16
+        uint8_t *d23 = (uint8_t *)Z.alloc(sec2_pts + L.size[3]);
+        R.device_scratch_bytes = Z.dev_bytes;
+        std::vector<uint8_t> s3(L.size[3]);
+        if (!zkey_pread(Z.fd, s3.data(), s3.size(), L.off[3])) return fail(POB_E_IO, std::string(who) + ": read error in section 3");
+        // the row side, on s_check while the reader starts
+        ZkeyCounters init{}; init.first_bad = ~0ull;
+        CU(cudaMemcpyAsync(ctr, &init, sizeof init, cudaMemcpyHostToDevice, Z.s_check));
+        CU(cudaMemsetAsync(coef_acc, 0, 64ull * slots, Z.s_check));
+        CU(cudaMemsetAsync(row_acc, 0, 64ull * slots, Z.s_check));
+        CU(cudaMemcpyAsync(d23, L.sec2 + ZK_SEC2_POINTS, sec2_pts, cudaMemcpyHostToDevice, Z.s_check));
+        CU(cudaMemcpyAsync(d23 + sec2_pts, s3.data(), s3.size(), cudaMemcpyHostToDevice, Z.s_check));
+        CU(cudaStreamSynchronize(Z.s_check));              // pageable sources: done before s3 and init go out of scope
+        cudaEvent_t r0 = Z.event(), r1 = Z.event();
+        CU(cudaEventRecord(r0, Z.s_check));
+        const unsigned gx = (unsigned)std::min<uint64_t>((nv + 255) / 256, h->n_sms * 16ull);
+        k_zkey_fill_x<<<gx, 256, 0, Z.s_check>>>(x, nv, seed);
+        for (uint64_t first = 0; first < m; first += W) {
+            const uint64_t cnt = std::min(W, m - first);
+            R1csArgs ra{C.flat, C.round, C.konst, (const uint64_t *)x, C.bases, first, cnt, wa, wb, nullptr};
+            k_r1cs_products<<<(unsigned)std::min<uint64_t>((2 * cnt + 255) / 256, h->n_sms * 16ull), 256, 0, Z.s_check>>>(ra);
+            k_zkey_rows<<<(unsigned)std::min<uint64_t>(slots, (cnt + 255) / 256), ZK_THREADS, 0, Z.s_check>>>(wa, wb, first, cnt, seed, row_acc);
+        }
+        // snarkjs's public rows m + s, a = x_s (s = 0 .. nPublic)
+        k_zkey_rows<<<1, ZK_THREADS, 0, Z.s_check>>>(x, nullptr, m, np + 1, seed, row_acc);
+        // the points of sections 2 and 3
+        const Fq b1 = zk_b1(); const Fq2 b2 = zk_b2();
+        const uint4 *p2 = (const uint4 *)d23;
+        const uint32_t sec2_off[6] = {0, 64, 128, 256, 384, 448};           // alpha1, beta1, beta2, gamma2, delta1, delta2
+        for (uint32_t i = 0; i < 6; i++) {
+            const uint4 *p = (const uint4 *)((const uint8_t *)p2 + sec2_off[i]);
+            if (i == 2 || i == 3 || i == 5) k_zkey_points<Fq2><<<1, ZK_THREADS, 0, Z.s_check>>>(p, 1, 2, i, b2, ctr);
+            else k_zkey_points<Fq><<<1, ZK_THREADS, 0, Z.s_check>>>(p, 1, 2, i, b1, ctr);
+        }
+        k_zkey_points<Fq><<<(unsigned)std::min<uint64_t>(slots, (np + 1 + 255) / 256), ZK_THREADS, 0, Z.s_check>>>(
+            (const uint4 *)(d23 + sec2_pts), np + 1, 3, 0, b1, ctr);
+        CU(cudaEventRecord(r1, Z.s_check));
+        R.points_checked = 6 + (np + 1);
+        for (auto [to, at, bytes] : {std::make_tuple((void *)dst->alpha1, 0u, 64u), std::make_tuple((void *)dst->beta1, 64u, 64u),
+                                     std::make_tuple((void *)dst->beta2, 128u, 128u), std::make_tuple((void *)dst->delta1, 384u, 64u),
+                                     std::make_tuple((void *)dst->delta2, 448u, 128u)})
+            CU(cudaMemcpyAsync(to, (const uint8_t *)p2 + at, bytes, cudaMemcpyDeviceToDevice, Z.s_check));
+        // sections 4..9 through the ring
+        Z.th = std::thread([&Z] { Z.reader(); });
+        std::vector<std::pair<cudaEvent_t, cudaEvent_t>> kpairs;
+        for (size_t j = 0; j < Z.jobs.size(); j++) {
+            const ZkeyLoad::Job &J = Z.jobs[j];
+            const int b = (int)(j % ZkeyLoad::NB);
+            {
+                std::unique_lock<std::mutex> l(Z.m);
+                Z.cv.wait(l, [&] { return Z.stop || Z.filled_upto > j; });
+                if (Z.filled_upto <= j) break;               // the reader stopped: an I/O error
+            }
+            if (J.section == 4) {
+                if (Z.k_rec[b]) { CU(cudaEventSynchronize(Z.k1[b])); R.check_ms += ZkeyLoad::elapsed(Z.k0[b], Z.k1[b]); Z.k_rec[b] = false; }
+                CU(cudaEventRecord(Z.c0[b], Z.s_copy));
+                CU(cudaMemcpyAsync(Z.dcoef[b], Z.pin[b], J.bytes, cudaMemcpyHostToDevice, Z.s_copy));
+                CU(cudaEventRecord(Z.c1[b], Z.s_copy));
+                CU(cudaStreamWaitEvent(Z.s_check, Z.c1[b], 0));
+                CU(cudaEventRecord(Z.k0[b], Z.s_check));
+                const uint64_t n = J.bytes / ZK_ENTRY_BYTES;
+                k_zkey_coefs<<<(unsigned)std::min<uint64_t>(slots, (n + 255) / 256), ZK_THREADS, 0, Z.s_check>>>(
+                    (const uint32_t *)Z.dcoef[b], n, x, nv, domain, seed, coef_acc, ctr);
+                CU(cudaEventRecord(Z.k1[b], Z.s_check));
+                Z.k_rec[b] = true;
+            } else {
+                CU(cudaEventRecord(Z.c0[b], Z.s_copy));
+                CU(cudaMemcpyAsync(dsec[J.section] + J.dst_off, Z.pin[b], J.bytes, cudaMemcpyHostToDevice, Z.s_copy));
+                CU(cudaEventRecord(Z.c1[b], Z.s_copy));
+                if (J.last) {                                // the whole section is in the key: check its points there
+                    CU(cudaStreamWaitEvent(Z.s_check, Z.c1[b], 0));
+                    const bool g2 = J.section == 7;
+                    const uint64_t n = L.size[J.section] / (g2 ? 128 : 64);
+                    cudaEvent_t e0 = Z.event(), e1 = Z.event();
+                    CU(cudaEventRecord(e0, Z.s_check));
+                    const unsigned g = (unsigned)std::min<uint64_t>(h->n_sms * 16ull, (n + 255) / 256);
+                    if (n && g2) k_zkey_points<Fq2><<<g, ZK_THREADS, 0, Z.s_check>>>((const uint4 *)dsec[7], n, 7, 0, b2, ctr);
+                    else if (n) k_zkey_points<Fq><<<g, ZK_THREADS, 0, Z.s_check>>>((const uint4 *)dsec[J.section], n, J.section, 0, b1, ctr);
+                    CU(cudaEventRecord(e1, Z.s_check));
+                    kpairs.emplace_back(e0, e1);
+                    R.points_checked += n;
+                }
+            }
+            CU(cudaGetLastError());
+            Z.c_rec[b] = true;
+            { std::lock_guard<std::mutex> l(Z.m); Z.state[b] = 0; }
+            Z.cv.notify_all();
+        }
+        Z.th.join();
+        if (!Z.cuda_err.empty()) return fail(POB_E_CUDA, std::string(who) + ": " + Z.cuda_err);
+        if (Z.io_err) return fail(POB_E_IO, std::string(who) + ": read error in " + path);
+        k_zkey_final<<<1, ZK_THREADS, 0, Z.s_check>>>(coef_acc, row_acc, slots, ctr);
+        CU(cudaGetLastError());
+        CU(cudaStreamSynchronize(Z.s_copy)); CU(cudaStreamSynchronize(Z.s_check));
+        for (int b = 0; b < ZkeyLoad::NB; b++) {
+            if (Z.c_rec[b]) Z.copy_ms += ZkeyLoad::elapsed(Z.c0[b], Z.c1[b]);
+            if (Z.k_rec[b]) R.check_ms += ZkeyLoad::elapsed(Z.k0[b], Z.k1[b]);
+        }
+        R.check_ms += ZkeyLoad::elapsed(r0, r1);
+        for (auto &p : kpairs) R.check_ms += ZkeyLoad::elapsed(p.first, p.second);
+        ZkeyCounters got{};
+        CU(cudaMemcpy(&got, ctr, sizeof got, cudaMemcpyDeviceToHost));
+        R.coef_match = got.match; R.coef_match_canonical = got.match_canonical; R.coef_out_of_range = got.out_of_range;
+        R.points_bad = got.points_bad; R.points_bad_canonical = got.points_bad_canonical;
+        if (got.first_bad != ~0ull) { R.first_bad_section = (uint32_t)(got.first_bad >> 40); R.first_bad_index = got.first_bad & ((1ull << 40) - 1); }
+        R.read_ms = (float)Z.read_ms; R.copy_ms = (float)Z.copy_ms;
+        R.bytes_read = ZK_SEC2_BYTES + L.size[3] + 4;
+        for (const ZkeyLoad::Job &J : Z.jobs) R.bytes_read += J.bytes;
+    } catch (const std::exception &e) { return fail(POB_E_CUDA, std::string(who) + ": " + e.what()); }
+    R.total_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_start).count();
+    if (rep) *rep = R;
+    std::string why;
+    for (int k = 0; k < 2; k++) if (!(R.coef_match >> k & 1))
+        why += std::string(why.empty() ? "" : "; ") + "matrix " + "AB"[k] + " of section 4 differs from the circuit's rows" +
+               ((R.coef_match_canonical >> k & 1) ? " (it matches with the values read as canonical elements, not c R^2)" : "");
+    if (R.coef_out_of_range) why += std::string(why.empty() ? "" : "; ") + std::to_string(R.coef_out_of_range) + " section-4 entries out of range";
+    if (R.points_bad)
+        why += std::string(why.empty() ? "" : "; ") + std::to_string(R.points_bad) + " points not on their curve, the first in section " +
+               std::to_string(R.first_bad_section) + " at index " + std::to_string(R.first_bad_index) +
+               (R.points_bad_canonical == 0 ? " (all pass with the coordinates read as canonical elements)" : "");
+    if (!why.empty()) return fail(POB_E_KEY, std::string(who) + ": the key does not fit the circuit: " + why);
+    return POB_OK;
+}

@@ -28,7 +28,7 @@ LIB_PATH = os.path.join(_HERE, "libpob_b200.so")
 
 RUN_EXPAND, RUN_DIGEST, RUN_INPUTS_STAGED, RUN_DISCARD = 1, 2, 4, 8
 CREATE_HCREATE, CREATE_O1 = 1, 0x100
-E_RANGE, E_REJECTED, E_BUSY, DONE = -5, -8, -9, 1
+E_RANGE, E_REJECTED, E_BUSY, E_KEY, DONE = -5, -8, -9, -10, 1
 MAIN_PROOF_OF_BURN = "ProofOfBurn(16, 4, 16, 50, 31, 2, 10 ** 19, 10 ** 20)"   # circuits/main_proof_of_burn.circom:27
 MAIN_SPEND = "Spend(31)"                                                       # circuits/main_spend.circom:6
 TEST_PROOF_OF_BURN = "ProofOfBurn(4, 4, 5, 20, 31, 2, 10 ** 18, 10 ** 19)"     # tests/testcases/proof_of_burn.py:53
@@ -96,6 +96,36 @@ class Groth16Key(collections.namedtuple("Groth16Key", "alpha1 beta1 delta1 beta2
     affine, Montgomery-form F_q limbs as msm_g1 / msm_g2 take them.  alpha1, beta1, delta1: one G1 point each; beta2, delta2: one G2
     point each; a, b1: n_signals G1 points; b2: n_signals G2 points; c: n_signals - n_outputs - 1 G1 points (wires n_outputs + 1 ..);
     h: 2^r1cs_domain() G1 points, paired with the quotient's q[k]."""
+
+
+class ZkeyDesc(ctypes.Structure):
+    """pob_b200.h: pob_zkey_desc"""
+    _fields_ = [("n_vars", ctypes.c_uint64), ("n_pub", ctypes.c_uint32), ("log_n", ctypes.c_uint32), ("n_coefs", ctypes.c_uint64),
+                ("file_bytes", ctypes.c_uint64), ("a_bytes", ctypes.c_uint64), ("b1_bytes", ctypes.c_uint64), ("b2_bytes", ctypes.c_uint64),
+                ("c_bytes", ctypes.c_uint64), ("h_bytes", ctypes.c_uint64), ("key_bytes", ctypes.c_uint64)]
+
+    def as_dict(self):
+        return {k: int(getattr(self, k)) for k, _ in self._fields_}
+
+
+class ZkeyReport(ctypes.Structure):
+    """pob_b200.h: pob_zkey_report"""
+    _fields_ = [("coef_match", ctypes.c_uint32), ("coef_match_canonical", ctypes.c_uint32), ("coef_out_of_range", ctypes.c_uint64),
+                ("points_checked", ctypes.c_uint64), ("points_bad", ctypes.c_uint64), ("points_bad_canonical", ctypes.c_uint64),
+                ("first_bad_section", ctypes.c_uint32), ("reserved", ctypes.c_uint32), ("first_bad_index", ctypes.c_uint64),
+                ("read_ms", ctypes.c_float), ("copy_ms", ctypes.c_float), ("check_ms", ctypes.c_float), ("total_ms", ctypes.c_float),
+                ("bytes_read", ctypes.c_uint64), ("device_scratch_bytes", ctypes.c_uint64)]
+
+    def as_dict(self):
+        return {k: (float(getattr(self, k)) if k.endswith("_ms") else int(getattr(self, k))) for k, _ in self._fields_ if k != "reserved"}
+
+
+class ZkeyError(PobError):
+    """a .zkey that does not fit the circuit (POB_E_KEY); .report is the check's report (a dict), None when it was refused on its header"""
+
+    def __init__(self, code, msg, report=None):
+        super().__init__(code, msg)
+        self.report = report
 
 
 class Proof(collections.namedtuple("Proof", "a b c")):
@@ -199,6 +229,10 @@ def lib():
         L.pob_groth16_work_bytes.argtypes = [vp, ctypes.POINTER(u64)]
         L.pob_groth16_prove.restype = ci
         L.pob_groth16_prove.argtypes = [vp, u32, ctypes.POINTER(Groth16KeyC), vp, vp, vp, vp, u64, vp]
+        L.pob_zkey_info.restype = ci
+        L.pob_zkey_info.argtypes = [ctypes.c_char_p, ctypes.POINTER(ZkeyDesc)]
+        L.pob_zkey_load.restype = ci
+        L.pob_zkey_load.argtypes = [vp, ctypes.c_char_p, u64, u64, ctypes.POINTER(Groth16KeyC), ctypes.POINTER(ZkeyReport)]
         L.pob_pow_grind.restype = ci
         L.pob_pow_grind.argtypes = [ci, vp, vp, vp, u32, u64, vp, ctypes.POINTER(u64)]
         L.pob_last_error.restype = ctypes.c_char_p
@@ -347,6 +381,17 @@ def write_r1cs(main_expr, path=None, hcreate=False, opt=0):
     d = R1csDesc()
     _check(lib().pob_write_r1cs(name.encode(), pl.ctypes.data, len(params), (CREATE_HCREATE if hcreate else 0) | (CREATE_O1 if opt else 0),
                                 None if path is None else os.fsencode(path), ctypes.byref(d)))
+    return d.as_dict()
+
+
+def zkey_info(path):
+    """header of a snarkjs `.zkey` (pob_zkey_info; host only, no GPU): n_vars, n_pub, log_n, n_coefs, file_bytes and the device bytes
+    of each key section.  A malformed file raises ZkeyError (E_KEY) or PobError (-6, I/O)."""
+    d = ZkeyDesc()
+    rc = lib().pob_zkey_info(os.fsencode(path), ctypes.byref(d))
+    if rc == E_KEY:
+        raise ZkeyError(rc, lib().pob_last_error().decode())
+    _check(rc)
     return d.as_dict()
 
 
@@ -621,6 +666,29 @@ class Circuit:
             return out
         return proof_from_limbs(out.cpu().tolist())
 
+    def load_zkey(self, path, seed=None, staging_bytes=0):
+        """the Groth16Key of a snarkjs `.zkey` (pob_zkey_load): the key tensors are allocated on this circuit's device and filled from
+        the file, which is checked against the circuit on the GPU on the way.  seed: of the coefficient check's random combination,
+        secrets.randbits(64) by default.  staging_bytes: pinned staging ring (0 = the library's default).  Returns (Groth16Key, report
+        dict); a key that does not fit raises ZkeyError with .report."""
+        import secrets
+        import torch
+        info = zkey_info(path)
+        seed = secrets.randbits(64) if seed is None else int(seed)
+        dev = torch.device("cuda", self.device)
+        n1 = lambda b, w: torch.empty((max(1, b // (8 * w)), w), dtype=torch.uint64, device=dev)    # a section of no points: one unused row
+        key = Groth16Key(alpha1=n1(64, 8), beta1=n1(64, 8), delta1=n1(64, 8), beta2=n1(128, 16), delta2=n1(128, 16), a=n1(info["a_bytes"], 8),
+                         b1=n1(info["b1_bytes"], 8), b2=n1(info["b2_bytes"], 16), c=n1(info["c_bytes"], 8), h=n1(info["h_bytes"], 8))
+        torch.cuda.synchronize(dev)
+        kc = Groth16KeyC(self.n_signals, self.n_outputs, self.r1cs_domain(), *[v.data_ptr() for v in key])
+        rep = ZkeyReport()
+        rc = lib().pob_zkey_load(self._h, os.fsencode(path), seed & ((1 << 64) - 1), int(staging_bytes), ctypes.byref(kc), ctypes.byref(rep))
+        if rc == E_KEY:
+            checked = rep.points_checked > 0
+            raise ZkeyError(rc, lib().pob_last_error().decode(), rep.as_dict() if checked else None)
+        _check(rc)
+        return key, rep.as_dict()
+
     def witness_map(self):
         m = np.zeros(self.n_signals, dtype=np.uint32)
         _check(lib().pob_witness_map(self._h, m.ctypes.data))
@@ -760,9 +828,47 @@ def main(argv=None):
     Batch form: `python -m pob_b200 <circuit> --batch in1.json in2.json ... --out DIR` evaluates all inputs in one
     pob_run_batch and writes DIR/<name>.wtns for every accepted instance.
     R1CS form: `python -m pob_b200 <circuit> --r1cs out.r1cs [--O1]` writes the circuit's `.r1cs` (host only, no GPU) in the wire
-    order of the --O0 witness, or of the reduced one with --O1."""
+    order of the --O0 witness, or of the reduced one with --O1.
+    Key check: `python -m pob_b200 <circuit> --check-zkey key.zkey [--O1]` loads a snarkjs `.zkey` and checks it against the circuit on
+    the GPU (Circuit.load_zkey); prints the report, exit code 1 when the key does not fit.
+    Proof: `python -m pob_b200 <circuit> --prove key.zkey input.json proof.json public.json [--O1]` generates the witness, loads and
+    checks the key, proves on the GPU and writes snarkjs-shaped proof.json and public.json; a rejected input or a key that does not
+    fit exits 1 and writes no proof."""
     import sys
     argv = sys.argv[1:] if argv is None else argv
+    if len(argv) in (3, 4) and argv[1] == "--check-zkey" and argv[3:] in ([], ["--O1"]):
+        c = Circuit(CIRCUIT_ALIASES.get(argv[0], argv[0]), max_slots=1, opt=1 if argv[3:] else 0)
+        try:
+            _, rep = c.load_zkey(argv[2])
+            print(json.dumps(dict(rep, ok=True)))
+            return 0
+        except ZkeyError as e:
+            print(json.dumps(dict(e.report or {}, ok=False)))
+            print(str(e), file=sys.stderr)
+            return 1
+        finally:
+            c.close()
+    if len(argv) in (6, 7) and argv[1] == "--prove" and argv[6:] in ([], ["--O1"]):
+        key_path, input_path, proof_path, public_path = argv[2:6]
+        c = Circuit(CIRCUIT_ALIASES.get(argv[0], argv[0]), max_slots=1, opt=1 if argv[6:] else 0)
+        try:
+            res = c.run([json.load(open(input_path))])
+            if res.status[0] != 0:
+                print("Error: constraint failed in the component at witness index %d" % (int(res.status[0]) - 1), file=sys.stderr)
+                return 1
+            try:
+                key, _ = c.load_zkey(key_path)
+            except ZkeyError as e:
+                print(str(e), file=sys.stderr)
+                return 1
+            proof = c.groth16_prove(0, key)
+            with open(proof_path, "w") as f:
+                json.dump(proof.to_json(), f)
+            with open(public_path, "w") as f:
+                json.dump(public_json(res.outputs[0]), f)
+            return 0
+        finally:
+            c.close()
     if len(argv) in (3, 4) and argv[1] == "--r1cs" and argv[3:] in ([], ["--O1"]):
         d = write_r1cs(CIRCUIT_ALIASES.get(argv[0], argv[0]), argv[2], opt=1 if argv[3:] else 0)
         print("%s: %d wires, %d constraints (%d non-linear), %d bytes" % (argv[2], d["n_wires"], d["n_constraints"], d["n_nonlinear"], d["file_bytes"]))
@@ -783,7 +889,9 @@ def main(argv=None):
     if len(argv) != 3:
         print("usage: python -m pob_b200 <main_proof_of_burn|main_spend|Template(params)> input.json witness.wtns\n"
               "       python -m pob_b200 <circuit> --batch in1.json in2.json ... --out DIR\n"
-              "       python -m pob_b200 <circuit> --r1cs out.r1cs [--O1]", file=sys.stderr)
+              "       python -m pob_b200 <circuit> --r1cs out.r1cs [--O1]\n"
+              "       python -m pob_b200 <circuit> --check-zkey key.zkey [--O1]\n"
+              "       python -m pob_b200 <circuit> --prove key.zkey input.json proof.json public.json [--O1]", file=sys.stderr)
         return 2
     c = Circuit(CIRCUIT_ALIASES.get(argv[0], argv[0]), max_slots=1)
     res = c.run([json.load(open(argv[1]))])
