@@ -392,6 +392,55 @@ typedef struct {
  * A failure of either part is POB_E_KEY with rep filled in (rep may be NULL). */
 int pob_zkey_load(pob_handle *h, const char *path, uint64_t seed, uint64_t staging_bytes, const pob_groth16_key *dst, pob_zkey_report *rep);
 
+/* the verification key of a .zkey (host-only, no GPU needed): alpha1 | beta2 | gamma2 | delta2 | IC copied byte for byte from sections 2
+ * and 3, 448 + 64 (n_pub + 1) bytes, Montgomery form as in the file; *n_pub = nPublic.  The file is validated exactly as pob_zkey_info
+ * does (same errors).  out_bytes shorter than the key: POB_E_BAD_ARG (with *n_pub set, so a caller can size out and call again). */
+int pob_zkey_vk(const char *path, void *out, uint64_t out_bytes, uint32_t *n_pub);
+
+/* ---- verification: the BN254 optimal ate pairing and Groth16 verdicts --------------------------------------------------------------
+ * e(P, Q) = f^((q^12 - 1) / r), the optimal ate pairing of BN254 (x = 4965661367192848881): the Miller loop over 6x + 2 and the lines
+ * at pi(Q) and -pi^2(Q), then the final exponentiation to exactly (q^12 - 1) / r (DESIGN.md §5 "Verification").  Values of F_q12 are
+ * 12 F_q elements in the nesting F_q12 = F_q6[w] / (w^2 - v), F_q6 = F_q2[v] / (v^3 - (9 + u)): c0.c0.c0, c0.c0.c1, c0.c1.c0, ..,
+ * c1.c2.c1, each a 32-byte LE CANONICAL element (the order of snarkjs's vk_alphabeta_12 as far as known here; not checked against
+ * snarkjs).  O on either side gives 1.
+ * pob_bn254_pairing: out[i] = e(g1[i], g2[i]), i < n.  g1: n x 64 B points as pob_msm_g1 bases, g2: n x 128 B as pob_msm_g2 bases
+ * (Montgomery form, all-zero = O), out: n x 384 B, all device memory.  The inputs are NOT checked to lie on their curves or in G1 / G2;
+ * outside them the value is not a pairing.  consumer_stream: NULL = return when done; else enqueued with no host wait and nothing
+ * allocated.  n == 0, a null or non-16-byte-aligned pointer, or out overlapping an input: POB_E_BAD_ARG before anything is enqueued. */
+int pob_bn254_pairing(int device, const void *g1, const void *g2, uint64_t n, void *out, void *consumer_stream);
+
+/* Groth16 verification, one verdict per proof: proof i is valid iff
+ *   e(-A_i, B_i) e(vk_x, gamma2) e(C_i, delta2) e(alpha1, beta2) == 1,   vk_x = IC_0 + sum_j pub_ij IC_j.
+ * vk     : device pointers, Montgomery form, affine, (0, 0) = O, as in a .zkey (pob_zkey_vk gives them in one buffer).
+ * proofs : n x 256 B, exactly what pob_groth16_prove writes: A (64 B), B (128 B), C (64 B), canonical affine, all-zero = O.
+ * publics: n x n_pub x 32 B canonical LE values; may be NULL when n_pub == 0.
+ * status : n x uint32 of device memory, one of POB_VERIFY_* below.  The checks run in this order and the first failure is reported:
+ *          a proof coordinate >= q or a point off its curve (BAD_POINT), a public input >= r (BAD_PUBLIC: never reduced, as on-chain
+ *          verifiers refuse it), B outside the order-r subgroup ([r]B != O: BAD_SUBGROUP), the equation (FAIL).  A = O or B = O is
+ *          not refused: its pairing is 1 and the equation decides.  A malformed key gives BAD_KEY to every proof of the call: a
+ *          coordinate >= q, a point off its curve, beta2, gamma2 or delta2 outside the subgroup, or gamma2 or delta2 = O.
+ * work   : caller scratch of pob_groth16_verify_work_bytes: the key's check flags, f_{alpha1,beta2} before its final exponentiation,
+ *          and the precomputed lines of gamma2 and delta2.
+ * consumer_stream: as pob_msm_g1 (NULL = return when done; else stream-ordered, no host wait, nothing allocated).
+ * A null pointer (publics only when n_pub > 0), a pointer that is not 16-byte aligned (status: 4-byte), a short work, n == 0, or
+ * status or work overlapping proofs, publics, a key point or each other: POB_E_BAD_ARG before anything is enqueued. */
+enum {
+    POB_VERIFY_OK = 0,              /* valid */
+    POB_VERIFY_FAIL = 1,            /* the pairing equation fails */
+    POB_VERIFY_BAD_POINT = 2,       /* a proof coordinate >= q, or a point off its curve */
+    POB_VERIFY_BAD_SUBGROUP = 3,    /* B outside the order-r subgroup */
+    POB_VERIFY_BAD_PUBLIC = 4,      /* a public input >= r */
+    POB_VERIFY_BAD_KEY = 5          /* the verification key is malformed (every proof of the call) */
+};
+typedef struct {
+    uint32_t n_pub;
+    const void *alpha1, *beta2, *gamma2, *delta2;  /* device, Montgomery, as in a .zkey: 64, 128, 128, 128 B */
+    const void *ic;                                 /* (n_pub + 1) G1 points, 64 B each */
+} pob_groth16_vk;
+int pob_groth16_verify_work_bytes(uint32_t n_pub, uint64_t n, uint64_t *bytes);   /* host-only, no GPU needed */
+int pob_groth16_verify(int device, const pob_groth16_vk *vk, const void *proofs, const void *publics, uint64_t n,
+                       uint32_t *status, void *work, uint64_t work_bytes, void *consumer_stream);
+
 /* ---- the step just before the path (SURVEY.md 8(f) rank 3) ------------------------------------------------------
  * replaces: find_burn_key() of the reference input generator (tests/main.py:47-56): starting at start_key, find the
  * first burnKey >= start_key whose keccak256(burnKey[32 BE] | revealAmount[32 BE] | burnExtraCommitment[32 BE] |

@@ -58,6 +58,15 @@ POB_HD bool f_is_zero(const Fq2 &a) { return fq2_is_zero(a); }
 POB_HD void f_set_zero(Fq2 &a) { a = fq2_zero(); }
 POB_HD void f_set_one(Fq2 &a) { a = fq2_one(); }
 
+// helpers of the pairing's tower (fq12_hd.h)
+POB_HD Fq2 fq2_conj(const Fq2 &a) { Fq2 r; r.c0 = a.c0; r.c1 = fq_neg(a.c1); return r; }          // a^q, the Frobenius of F_q2
+POB_HD Fq2 fq2_mul_fq(const Fq2 &a, const Fq &k) { Fq2 r; r.c0 = fq_mul(a.c0, k); r.c1 = fq_mul(a.c1, k); return r; }
+// a xi with xi = 9 + u: (9 a0 - a1) + (9 a1 + a0) u, by additions
+POB_HD Fq2 fq2_mul_xi(const Fq2 &a) {
+    const Fq2 a2 = fq2_add(a, a), a4 = fq2_add(a2, a2), a8 = fq2_add(a4, a4), a9 = fq2_add(a8, a);
+    Fq2 r; r.c0 = fq_sub(a9.c0, a.c1); r.c1 = fq_add(a9.c1, a.c0); return r;
+}
+
 typedef Aff<Fq2> G2Aff;      // 128 bytes: x.c0, x.c1, y.c0, y.c1
 typedef Xyzz<Fq2> G2Xyzz;
 

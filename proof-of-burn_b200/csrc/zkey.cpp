@@ -115,3 +115,23 @@ int pob_zkey_info(const char *path, pob_zkey_desc *out) {
     catch (const pob::ZkeyError &e) { pob_set_error(std::string("pob_zkey_info: ") + path + ": " + e.what()); return e.code; }
     return POB_OK;
 }
+
+extern "C" int pob_zkey_vk(const char *path, void *out, uint64_t out_bytes, uint32_t *n_pub);
+
+int pob_zkey_vk(const char *path, void *out, uint64_t out_bytes, uint32_t *n_pub) {
+    if (!path || !out || !n_pub) { pob_set_error("pob_zkey_vk: null argument"); return POB_E_BAD_ARG; }
+    try {
+        const pob::ZkeyLayout L = pob::zkey_parse(path);
+        *n_pub = L.n_pub;
+        const uint64_t need = 448 + L.size[3];
+        if (out_bytes < need) { pob_set_error("pob_zkey_vk: out holds " + std::to_string(out_bytes) + " bytes, the key has " + std::to_string(need)); return POB_E_BAD_ARG; }
+        uint8_t *o = (uint8_t *)out;
+        const uint8_t *s2 = L.sec2 + 84;                                   // alpha1, beta1, beta2, gamma2, delta1, delta2
+        memcpy(o, s2, 64);                                                 // alpha1
+        memcpy(o + 64, s2 + 128, 256);                                     // beta2, gamma2
+        memcpy(o + 320, s2 + 448, 128);                                    // delta2
+        pob::Fd f(open(path, O_RDONLY));
+        if (f.fd < 0 || !pob::zkey_pread(f.fd, o + 448, L.size[3], L.off[3])) { pob_set_error(std::string("pob_zkey_vk: ") + path + ": read error in section 3"); return POB_E_IO; }
+    } catch (const pob::ZkeyError &e) { pob_set_error(std::string("pob_zkey_vk: ") + path + ": " + e.what()); return e.code; }
+    return POB_OK;
+}

@@ -23,12 +23,14 @@ import numpy as np
 
 P = 21888242871839275222246405745257275088548364400416034343698204186575808495617
 R_ORDER = P                                       # BN254's group order r is the scalar field's modulus
+Q = 21888242871839275222246405745257275088696311157297823662689037894645226208583   # BN254's base field modulus
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libpob_b200.so")
 
 RUN_EXPAND, RUN_DIGEST, RUN_INPUTS_STAGED, RUN_DISCARD = 1, 2, 4, 8
 CREATE_HCREATE, CREATE_O1 = 1, 0x100
 E_RANGE, E_REJECTED, E_BUSY, E_KEY, DONE = -5, -8, -9, -10, 1
+VERIFY_STATUS = ("OK", "FAIL", "BAD_POINT", "BAD_SUBGROUP", "BAD_PUBLIC", "BAD_KEY")    # pob_b200.h: POB_VERIFY_*, by value
 MAIN_PROOF_OF_BURN = "ProofOfBurn(16, 4, 16, 50, 31, 2, 10 ** 19, 10 ** 20)"   # circuits/main_proof_of_burn.circom:27
 MAIN_SPEND = "Spend(31)"                                                       # circuits/main_spend.circom:6
 TEST_PROOF_OF_BURN = "ProofOfBurn(4, 4, 5, 20, 31, 2, 10 ** 18, 10 ** 19)"     # tests/testcases/proof_of_burn.py:53
@@ -120,6 +122,11 @@ class ZkeyReport(ctypes.Structure):
         return {k: (float(getattr(self, k)) if k.endswith("_ms") else int(getattr(self, k))) for k, _ in self._fields_ if k != "reserved"}
 
 
+class Groth16VkC(ctypes.Structure):
+    """pob_b200.h: pob_groth16_vk"""
+    _fields_ = [("n_pub", ctypes.c_uint32)] + [(f, ctypes.c_void_p) for f in ("alpha1", "beta2", "gamma2", "delta2", "ic")]
+
+
 class ZkeyError(PobError):
     """a .zkey that does not fit the circuit (POB_E_KEY); .report is the check's report (a dict), None when it was refused on its header"""
 
@@ -134,14 +141,40 @@ class Proof(collections.namedtuple("Proof", "a b c")):
     def to_json(self):
         """the proof.json dictionary of snarkjs (pi_a, pi_b, pi_c as projective decimal strings with z = 1, pi_b coordinates as
         [c0, c1]).  The shape follows snarkjs as far as it is known here; it has not been checked against snarkjs."""
-        def g1(p):
-            return ["0", "1", "0"] if p is None else [str(p[0]), str(p[1]), "1"]
+        return {"pi_a": _g1_json(self.a), "pi_b": _g2_json(self.b), "pi_c": _g1_json(self.c), "protocol": "groth16", "curve": "bn128"}
 
-        def g2(p):
-            if p is None:
-                return [["0", "0"], ["1", "0"], ["0", "0"]]
-            return [[str(p[0][0]), str(p[0][1])], [str(p[1][0]), str(p[1][1])], ["1", "0"]]
-        return {"pi_a": g1(self.a), "pi_b": g2(self.b), "pi_c": g1(self.c), "protocol": "groth16", "curve": "bn128"}
+    @classmethod
+    def from_json(cls, d):
+        """the inverse of to_json: z = 1, or the infinity encodings to_json writes; anything else raises ValueError"""
+        return cls(_g1_from_json(d["pi_a"]), _g2_from_json(d["pi_b"]), _g1_from_json(d["pi_c"]))
+
+
+def _g1_json(p):
+    return ["0", "1", "0"] if p is None else [str(p[0]), str(p[1]), "1"]
+
+
+def _g2_json(p):
+    if p is None:
+        return [["0", "0"], ["1", "0"], ["0", "0"]]
+    return [[str(p[0][0]), str(p[0][1])], [str(p[1][0]), str(p[1][1])], ["1", "0"]]
+
+
+def _g1_from_json(v):
+    v = [str(x) for x in v]
+    if v == ["0", "1", "0"]:
+        return None
+    if len(v) != 3 or v[2] != "1":
+        raise ValueError("a G1 point must be [x, y, 1] or [0, 1, 0] (infinity): %r" % (v,))
+    return (int(v[0]), int(v[1]))
+
+
+def _g2_from_json(v):
+    v = [[str(x) for x in c] for c in v]
+    if v == [["0", "0"], ["1", "0"], ["0", "0"]]:
+        return None
+    if len(v) != 3 or any(len(c) != 2 for c in v) or v[2] != ["1", "0"]:
+        raise ValueError("a G2 point must be [[x0, x1], [y0, y1], [1, 0]] or [[0, 0], [1, 0], [0, 0]] (infinity): %r" % (v,))
+    return ((int(v[0][0]), int(v[0][1])), (int(v[1][0]), int(v[1][1])))
 
 
 def public_json(outputs):
@@ -233,6 +266,14 @@ def lib():
         L.pob_zkey_info.argtypes = [ctypes.c_char_p, ctypes.POINTER(ZkeyDesc)]
         L.pob_zkey_load.restype = ci
         L.pob_zkey_load.argtypes = [vp, ctypes.c_char_p, u64, u64, ctypes.POINTER(Groth16KeyC), ctypes.POINTER(ZkeyReport)]
+        L.pob_zkey_vk.restype = ci
+        L.pob_zkey_vk.argtypes = [ctypes.c_char_p, vp, u64, ctypes.POINTER(u32)]
+        L.pob_bn254_pairing.restype = ci
+        L.pob_bn254_pairing.argtypes = [ci, vp, vp, u64, vp, vp]
+        L.pob_groth16_verify_work_bytes.restype = ci
+        L.pob_groth16_verify_work_bytes.argtypes = [u32, u64, ctypes.POINTER(u64)]
+        L.pob_groth16_verify.restype = ci
+        L.pob_groth16_verify.argtypes = [ci, ctypes.POINTER(Groth16VkC), vp, vp, u64, vp, vp, u64, vp]
         L.pob_pow_grind.restype = ci
         L.pob_pow_grind.argtypes = [ci, vp, vp, vp, u32, u64, vp, ctypes.POINTER(u64)]
         L.pob_last_error.restype = ctypes.c_char_p
@@ -802,6 +843,209 @@ def msm_g2(bases, scalars, stream=None, out=None, work=None, device=None):
     return None if c is None else ((c[0], c[1]), (c[2], c[3]))
 
 
+# ---- verification (pob_bn254_pairing, pob_groth16_verify) -----------------------------------------------------------------------
+_RM = 1 << 256
+
+
+def _fq_bytes(v, mont):
+    """32 LE bytes of an F_q coordinate: its Montgomery form (v must be canonical, 0 <= v < q: a key's point is never reduced), or
+    v itself unchanged (a proof's coordinate, which the device range-checks)"""
+    v = int(v)
+    if mont and not 0 <= v < Q:
+        raise ValueError("a key coordinate must lie in [0, q): %d" % v)
+    return (v * _RM % Q if mont else v).to_bytes(32, "little")
+
+
+def _enc_g1(p, mont):
+    return bytes(64) if p is None else _fq_bytes(p[0], mont) + _fq_bytes(p[1], mont)
+
+
+def _enc_g2(p, mont):
+    return bytes(128) if p is None else b"".join(_fq_bytes(v, mont) for v in (p[0][0], p[0][1], p[1][0], p[1][1]))
+
+
+def _u64(raw, width):
+    return np.frombuffer(raw, dtype=np.uint64).reshape(-1, width).copy()
+
+
+def _to_dev(arr, dev):
+    """a uint64 numpy array as a uint64 CUDA tensor, copied on the current stream from a pinned staging buffer (no host wait; the
+    caching host allocator keeps the buffer until the copy is done)"""
+    import torch
+    return torch.from_numpy(arr.view(np.int64)).pin_memory().to(dev, non_blocking=True).view(torch.uint64)
+
+
+def _dec_fq(raw, mont):
+    v = int.from_bytes(raw, "little")
+    return v * pow(_RM, -1, Q) % Q if mont else v
+
+
+def _dec_g1(raw, mont):
+    return None if not any(raw) else (_dec_fq(raw[:32], mont), _dec_fq(raw[32:64], mont))
+
+
+def _dec_g2(raw, mont):
+    if not any(raw):
+        return None
+    c = [_dec_fq(raw[32 * k:32 * k + 32], mont) for k in range(4)]
+    return ((c[0], c[1]), (c[2], c[3]))
+
+
+def _stream_ctx(dev, handle):
+    import torch
+    return torch.cuda.stream(torch.cuda.ExternalStream(handle, device=dev) if handle else torch.cuda.current_stream(dev))
+
+
+def pairing(g1_points, g2_points, device=0):
+    """[e(P_i, Q_i)] on the GPU (pob_bn254_pairing): P_i G1 points (x, y), Q_i G2 points ((x0, x1), (y0, y1)), canonical ints, None =
+    infinity; not checked to lie in G1 / G2.  Each value is a 12-tuple of ints in vk_alphabeta_12's nesting (c0.c0.c0, c0.c0.c1, ..)."""
+    import torch
+    n = len(g1_points)
+    if n == 0 or len(g2_points) != n:
+        raise ValueError("pairing: need equally many (>= 1) G1 and G2 points")
+    dev = torch.device("cuda", device)
+    a = _to_dev(_u64(b"".join(_enc_g1(p, True) for p in g1_points), 8), dev)
+    b = _to_dev(_u64(b"".join(_enc_g2(p, True) for p in g2_points), 16), dev)
+    out = torch.empty((n, 48), dtype=torch.uint64, device=dev)
+    torch.cuda.synchronize(dev)
+    _check(lib().pob_bn254_pairing(dev.index, a.data_ptr(), b.data_ptr(), n, out.data_ptr(), None))
+    raw = out.view(torch.int64).cpu().numpy().tobytes()
+    return [tuple(int.from_bytes(raw[384 * i + 32 * k:384 * i + 32 * k + 32], "little") for k in range(12)) for i in range(n)]
+
+
+class DeviceVerificationKey(collections.namedtuple("DeviceVerificationKey", "n_pub alpha1 beta2 gamma2 delta2 ic")):
+    """A verification key as CUDA tensors (pob_b200.h: pob_groth16_vk): alpha1 (1, 8), beta2, gamma2, delta2 (1, 16) and ic
+    (n_pub + 1, 8) uint64, affine Montgomery form as in a .zkey."""
+
+
+class VerificationKey(collections.namedtuple("VerificationKey", "alpha1 beta2 gamma2 delta2 ic")):
+    """A Groth16 verification key of ints: alpha1 and the IC points (a list of n_pub + 1) are G1 points (x, y), beta2, gamma2 and
+    delta2 G2 points ((x0, x1), (y0, y1)); None = infinity."""
+
+    @property
+    def n_pub(self):
+        return len(self.ic) - 1
+
+    @classmethod
+    def from_zkey(cls, path):
+        """sections 2 and 3 of a snarkjs `.zkey` (pob_zkey_vk; host only, no GPU).  A malformed file raises ZkeyError or PobError."""
+        n_pub = ctypes.c_uint32(0)
+        rc = lib().pob_zkey_vk(os.fsencode(path), ctypes.create_string_buffer(1), 1, ctypes.byref(n_pub))   # short: sizes the key
+        if rc == E_KEY:
+            raise ZkeyError(rc, lib().pob_last_error().decode())
+        if rc != -1:
+            _check(rc)
+        buf = ctypes.create_string_buffer(448 + 64 * (n_pub.value + 1))
+        rc = lib().pob_zkey_vk(os.fsencode(path), buf, len(buf), ctypes.byref(n_pub))
+        if rc == E_KEY:
+            raise ZkeyError(rc, lib().pob_last_error().decode())
+        _check(rc)
+        raw = buf.raw
+        ic = [_dec_g1(raw[448 + 64 * k:512 + 64 * k], True) for k in range(n_pub.value + 1)]
+        return cls(_dec_g1(raw[:64], True), _dec_g2(raw[64:192], True), _dec_g2(raw[192:320], True), _dec_g2(raw[320:448], True), ic)
+
+    @classmethod
+    def from_json(cls, d):
+        """from snarkjs's verification_key.json shape (to_json); vk_alphabeta_12 is ignored (verification recomputes it)"""
+        if d.get("protocol", "groth16") != "groth16" or d.get("curve", "bn128") != "bn128":
+            raise ValueError("not a Groth16 BN254 verification key")
+        ic = [_g1_from_json(p) for p in d["IC"]]
+        if "nPublic" in d and int(d["nPublic"]) != len(ic) - 1:
+            raise ValueError("nPublic is %s but IC has %d points" % (d["nPublic"], len(ic)))
+        vk = cls(_g1_from_json(d["vk_alpha_1"]), _g2_from_json(d["vk_beta_2"]), _g2_from_json(d["vk_gamma_2"]),
+                 _g2_from_json(d["vk_delta_2"]), ic)
+        for p in [vk.alpha1] + list(vk.ic):
+            if p is not None and not all(0 <= v < Q for v in p):
+                raise ValueError("a G1 coordinate of the key is not in [0, q): %r" % (p,))
+        for p in (vk.beta2, vk.gamma2, vk.delta2):
+            if p is not None and not all(0 <= v < Q for c in p for v in c):
+                raise ValueError("a G2 coordinate of the key is not in [0, q): %r" % (p,))
+        return vk
+
+    def to_json(self, device=0):
+        """snarkjs's verification_key.json dictionary, as far as its shape is known here; vk_alphabeta_12 = e(alpha1, beta2) from
+        pob_bn254_pairing, nested [[[c000, c001], [c010, c011], [c020, c021]], [[c100, ..], ..]]"""
+        e = pairing([self.alpha1], [self.beta2], device=device)[0]
+        ab = [[[str(e[6 * h + 2 * j]), str(e[6 * h + 2 * j + 1])] for j in range(3)] for h in range(2)]
+        return {"protocol": "groth16", "curve": "bn128", "nPublic": self.n_pub, "vk_alpha_1": _g1_json(self.alpha1),
+                "vk_beta_2": _g2_json(self.beta2), "vk_gamma_2": _g2_json(self.gamma2), "vk_delta_2": _g2_json(self.delta2),
+                "vk_alphabeta_12": ab, "IC": [_g1_json(p) for p in self.ic]}
+
+    def to_device(self, device=0):
+        """the DeviceVerificationKey of this key on cuda:device"""
+        import torch
+        dev = torch.device("cuda", device)
+        raw = [(_enc_g1(self.alpha1, True), 8), (_enc_g2(self.beta2, True), 16), (_enc_g2(self.gamma2, True), 16),
+               (_enc_g2(self.delta2, True), 16), (b"".join(_enc_g1(p, True) for p in self.ic), 8)]      # every coordinate checked first
+        return DeviceVerificationKey(self.n_pub, *[_to_dev(_u64(r, w), dev) for r, w in raw])
+
+
+def groth16_verify_work_bytes(n_pub, n):
+    """bytes of scratch pob_groth16_verify needs (host only, no GPU)"""
+    v = ctypes.c_uint64(0)
+    _check(lib().pob_groth16_verify_work_bytes(int(n_pub), int(n), ctypes.byref(v)))
+    return int(v.value)
+
+
+def groth16_verify(vk, proofs, publics, device=0, stream=None, status=None, work=None):
+    """Groth16 verdicts on the GPU (pob_groth16_verify), one per proof: 0 valid, else a VERIFY_STATUS code.
+    vk: VerificationKey or DeviceVerificationKey.  proofs: a list of Proof, or a CUDA uint64 tensor of (32,) or (n, 32) limbs as
+    Circuit.groth16_prove's out.  publics: a list of n lists of n_pub ints (values >= r are passed through unreduced and refused), or
+    a CUDA uint64 tensor of n x n_pub x 4 limbs.  status: an optional CUDA int32 / uint32 tensor of >= n elements; work: an optional
+    CUDA tensor of >= groth16_verify_work_bytes bytes.  Returns a numpy uint32 array; with a stream (torch.cuda.Stream or raw
+    cudaStream_t) everything, the key's and the host inputs' transfers included (through pinned staging buffers), is enqueued on it
+    with no host wait, and the (n,) status tensor is returned unsynchronised."""
+    import torch
+    handle = None if stream is None else getattr(stream, "cuda_stream", stream)
+    if isinstance(proofs, torch.Tensor):
+        dev = proofs.device
+        if not proofs.is_cuda or not proofs.is_contiguous() or proofs.numel() % 32 or proofs.element_size() != 8:
+            raise ValueError("groth16_verify: proofs must be a contiguous CUDA uint64 tensor of n x 32 limbs")
+        n = proofs.numel() // 32
+    else:
+        dev = torch.device("cuda", device)
+        n = len(proofs)
+    if n == 0:
+        raise ValueError("groth16_verify: no proofs")
+    n_pub = vk.n_pub
+    with _stream_ctx(dev, handle):                  # every temporary is allocated on the stream that uses it
+        if isinstance(vk, VerificationKey):
+            vk = vk.to_device(dev.index)
+        if not isinstance(proofs, torch.Tensor):
+            raw = b"".join(_enc_g1(p.a, False) + _enc_g2(p.b, False) + _enc_g1(p.c, False) for p in proofs)
+            proofs = _to_dev(_u64(raw, 32), dev)
+        pub_t = None
+        if isinstance(publics, torch.Tensor):
+            if publics.device != dev or not publics.is_contiguous() or publics.numel() != 4 * n_pub * n or publics.element_size() != 8:
+                raise ValueError("groth16_verify: publics must be a contiguous CUDA uint64 tensor of n x n_pub x 4 limbs")
+            pub_t = publics
+        elif n_pub:
+            if len(publics) != n or any(len(v) != n_pub for v in publics):
+                raise ValueError("groth16_verify: need n_pub = %d public inputs for each of %d proofs" % (n_pub, n))
+            if any(not 0 <= int(x) < 1 << 256 for v in publics for x in v):
+                raise ValueError("groth16_verify: a public input must be a 256-bit unsigned integer")
+            pub_t = _to_dev(_u64(b"".join(int(x).to_bytes(32, "little") for v in publics for x in v), 4), dev)
+        if status is None:
+            status = torch.empty(n, dtype=torch.int32, device=dev)
+        if work is None:
+            work = torch.empty(groth16_verify_work_bytes(n_pub, n), dtype=torch.uint8, device=dev)
+    key_bytes = {"alpha1": 64, "beta2": 128, "gamma2": 128, "delta2": 128, "ic": 64 * (n_pub + 1)}
+    for t, what, need in [(status, "status", 4 * n), (work, "work", groth16_verify_work_bytes(n_pub, n))] + \
+            [(getattr(vk, f), "vk." + f, b) for f, b in key_bytes.items()]:
+        if not isinstance(t, torch.Tensor) or t.device != dev or not t.is_contiguous() or t.numel() * t.element_size() < need:
+            raise ValueError("groth16_verify: %s must be a contiguous tensor on %s of at least %d bytes" % (what, dev, need))
+    if status.element_size() != 4:
+        raise ValueError("groth16_verify: status must hold 32-bit elements")
+    kc = Groth16VkC(n_pub, *[t.data_ptr() for t in (vk.alpha1, vk.beta2, vk.gamma2, vk.delta2, vk.ic)])
+    if handle is None:
+        torch.cuda.synchronize(dev)
+    _check(lib().pob_groth16_verify(dev.index, ctypes.byref(kc), proofs.data_ptr(), None if pub_t is None else pub_t.data_ptr(), n,
+                                    status.data_ptr(), work.data_ptr(), work.numel() * work.element_size(), handle))
+    if handle:
+        return status
+    return status[:n].cpu().numpy().astype(np.uint32)
+
+
 def repad_pob_input(inp, max_layers, node_blocks, header_blocks):
     """Re-pad a ProofOfBurn input JSON to a circuit shape: unused layers are zero with length 256 (the convention of
     reference tests/main.py:148-150), the header is zero-extended.  The reference generator still pads to the (4,.,5)
@@ -833,9 +1077,40 @@ def main(argv=None):
     the GPU (Circuit.load_zkey); prints the report, exit code 1 when the key does not fit.
     Proof: `python -m pob_b200 <circuit> --prove key.zkey input.json proof.json public.json [--O1]` generates the witness, loads and
     checks the key, proves on the GPU and writes snarkjs-shaped proof.json and public.json; a rejected input or a key that does not
-    fit exits 1 and writes no proof."""
+    fit exits 1 and writes no proof.
+    Verification key: `python -m pob_b200 --export-vk key.zkey verification_key.json` writes snarkjs's verification_key.json shape
+    from the .zkey (vk_alphabeta_12 computed on the GPU).
+    Verification: `python -m pob_b200 --verify verification_key.json public.json proof.json [public2.json proof2.json ...]` (snarkjs's
+    argument order) verifies every pair in one GPU call, prints one line per pair (OK or the status's name) and exits 0 only when
+    every proof is valid, else 1."""
     import sys
     argv = sys.argv[1:] if argv is None else argv
+    if len(argv) == 3 and argv[0] == "--export-vk":
+        vk = VerificationKey.from_zkey(argv[1])
+        with open(argv[2], "w") as f:
+            json.dump(vk.to_json(), f, indent=1)
+        return 0
+    if len(argv) >= 4 and len(argv) % 2 == 0 and argv[0] == "--verify":
+        with open(argv[1]) as f:
+            try:
+                vk = VerificationKey.from_json(json.load(f))
+            except ValueError as e:
+                print("%s: %s" % (argv[1], e), file=sys.stderr)
+                return 1
+        pairs = [(argv[k], argv[k + 1]) for k in range(2, len(argv), 2)]
+        publics, proofs = [], []
+        for pub_path, proof_path in pairs:
+            with open(pub_path) as f:
+                publics.append([int(v) for v in json.load(f)])
+            with open(proof_path) as f:
+                proofs.append(Proof.from_json(json.load(f)))
+        if any(len(p) != vk.n_pub for p in publics):
+            print("a public.json does not hold nPublic = %d values" % vk.n_pub, file=sys.stderr)
+            return 1
+        status = groth16_verify(vk, proofs, publics)
+        for (pub_path, proof_path), s in zip(pairs, status):
+            print("%s %s: %s" % (pub_path, proof_path, VERIFY_STATUS[int(s)]))
+        return 0 if all(int(s) == 0 for s in status) else 1
     if len(argv) in (3, 4) and argv[1] == "--check-zkey" and argv[3:] in ([], ["--O1"]):
         c = Circuit(CIRCUIT_ALIASES.get(argv[0], argv[0]), max_slots=1, opt=1 if argv[3:] else 0)
         try:
@@ -886,12 +1161,14 @@ def main(argv=None):
                 print("%s: constraint failed in the component at witness index %d" % (f, int(res.status[i]) - 1), file=sys.stderr)
                 rc = 1
         return rc
-    if len(argv) != 3:
+    if len(argv) != 3 or argv[0] in ("--export-vk", "--verify"):
         print("usage: python -m pob_b200 <main_proof_of_burn|main_spend|Template(params)> input.json witness.wtns\n"
               "       python -m pob_b200 <circuit> --batch in1.json in2.json ... --out DIR\n"
               "       python -m pob_b200 <circuit> --r1cs out.r1cs [--O1]\n"
               "       python -m pob_b200 <circuit> --check-zkey key.zkey [--O1]\n"
-              "       python -m pob_b200 <circuit> --prove key.zkey input.json proof.json public.json [--O1]", file=sys.stderr)
+              "       python -m pob_b200 <circuit> --prove key.zkey input.json proof.json public.json [--O1]\n"
+              "       python -m pob_b200 --export-vk key.zkey verification_key.json\n"
+              "       python -m pob_b200 --verify verification_key.json public.json proof.json [public2.json proof2.json ...]", file=sys.stderr)
         return 2
     c = Circuit(CIRCUIT_ALIASES.get(argv[0], argv[0]), max_slots=1)
     res = c.run([json.load(open(argv[1]))])
